@@ -42,10 +42,10 @@ struct IntraParams {
 __device__ __forceinline__ int wide_angle(int w, int h, int mode)
 {
   if (mode > 1 && mode <= 66) {
-    const int shift[6] = {0, 6, 10, 12, 14, 15};
     const int d = abs((31 - __clz(w)) - (31 - __clz(h)));
-    if (w > h && mode < 2 + shift[d]) mode += 65;
-    else if (h > w && mode > 66 - shift[d]) mode -= 65;
+    const int shift = (int)((0x0F0E0C0A0600ull >> (8 * d)) & 0xff);   // {0, 6, 10, 12, 14, 15}[d], in a register rather than a local array
+    if (w > h && mode < 2 + shift) mode += 65;
+    else if (h > w && mode > 66 - shift) mode -= 65;
   }
   return mode;
 }
@@ -461,7 +461,7 @@ constexpr int V2_LS = 136, V2_CS = 72;                       // tile row pitch i
 constexpr int V2_TILE = 128 * V2_LS + 2 * 64 * V2_CS;        // samples of one tile set (Y, Cb, Cr)
 constexpr int V2_RECS = 1024;                                // records staged in shared memory (a CTU with more blocks reads the rest from global memory)
 constexpr int V2_FLAGS = 128 * 128 / 16 + 2 * (64 * 64 / 4); // most blocks a CTU can hold
-struct V2Scratch { int16_t T[2][IT_REF], L[2][IT_REF], M[IT_ARR], S[IT_ARR], Lm[32 * 32], LmTop[64], LmLeft[64]; int LmPar[4]; int ticket, sum; };
+struct V2Scratch { int16_t T[2][IT_REF], L[2][IT_REF], M[IT_ARR], S[IT_ARR], Lm[32 * 32], LmTop[64], LmLeft[64]; int LmPar[4]; int next[2], sum; };
 constexpr int V2_OWN = 3 * 32 * 32;                         // owner words of the CTU's units: luma 32 x 32 (4x4 units), Cb / Cr 32 x 32 each (2x2 units)
 constexpr size_t v2_smem(int groups) { return (size_t)2 * V2_TILE * sizeof(int16_t) + groups * sizeof(V2Scratch) + V2_RECS * sizeof(b200_intra_tu) + V2_OWN * sizeof(int) + V2_FLAGS + 64; }
 __device__ __forceinline__ void v2_cp4(void* smemDst, const void* gmemSrc)      // asynchronous 4-byte global -> shared copy (LDGSTS): the whole CTU in flight before one wait
@@ -476,16 +476,7 @@ __device__ __forceinline__ void v2_cp16(void* smemDst, const void* gmemSrc)
 }
 __device__ __forceinline__ void v2_cp_wait() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 
-struct V2Tile {
-  int16_t* rec[3]; int16_t* res[3]; int ox[3], oy[3], tw[3], th[3], ts[3];
-  const int16_t* plane[3]; int ps[3];
-  __device__ __forceinline__ bool inside(int c, int x, int y) const { return (unsigned)(x - ox[c]) < (unsigned)tw[c] && (unsigned)(y - oy[c]) < (unsigned)th[c]; }
-  __device__ __forceinline__ int pix(int c, int x, int y) const
-  {
-    if (inside(c, x, y)) return rec[c][(y - oy[c]) * ts[c] + (x - ox[c])];
-    return __ldcg(plane[c] + (size_t)y * ps[c] + x);
-  }
-};
+__device__ __forceinline__ int v2_tile_off(int c) { return c == 0 ? 0 : c == 1 ? 128 * V2_LS : 128 * V2_LS + 64 * V2_CS; }     // component c in a tile set
 
 // CTUs that hold blocks, sorted by the wave-front key (x + 2 y, then y): every CTU counts the non-empty CTUs that precede it
 __global__ void __launch_bounds__(1024) intra_ctu_order_kernel(const IntraParams P, int* ctuOrder, int* counters)
@@ -512,15 +503,22 @@ __global__ void __launch_bounds__(256) intra_ctu_check_kernel(const IntraParams 
   if (i - P.ctuFirst[c] >= P.ctuCnt[c]) atomicOr(P.err, 2);
 }
 
-// returns true if the block waited for lives in another CTU (its samples are then read from the plane: a device-scope fence is due)
-__device__ __forceinline__ bool v2_wait(const IntraParams& P, const volatile uint8_t* sflag, int o, int me, int first)
+__device__ __forceinline__ int v2_ld_acquire(const int* p) { int v; asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
+__device__ __forceinline__ void v2_st_release(int* p, int v) { asm volatile("st.release.gpu.global.b32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
+
+// waits for block o (if it is an earlier block) with acquire semantics: the calling thread's group barrier after the waits orders the group's reads of the
+// block's samples behind it — shared-memory done bytes for blocks of this CTU (CTA scope), the global done words for the others (GPU scope)
+__device__ __forceinline__ void v2_wait(const IntraParams& P, const volatile uint8_t* sflag, int o, int me, int first)
 {
-  if (o < 0 || o >= me) return false;
+  if (o < 0 || o >= me) return;
   int spins = 0;
-  if (o >= first) { while (sflag[o - first] == 0) { if (++spins > 64) __nanosleep(20); if (spins > (1 << 24)) { atomicOr(P.err, 1); break; } } return false; }
-  const volatile int* d = P.done + o; const volatile int* e = P.err;
-  while (*d == 0) { __nanosleep(32); if (*e || ++spins > (1 << 22)) { atomicOr(P.err, 1); break; } }
-  return true;
+  if (o >= first) {
+    while (sflag[o - first] == 0) { if (++spins > 64) __nanosleep(20); if (spins > (1 << 24)) { atomicOr(P.err, 1); break; } }
+    __threadfence_block();
+    return;
+  }
+  const volatile int* e = P.err;
+  while (v2_ld_acquire(P.done + o) == 0) { __nanosleep(32); if (*e || ++spins > (1 << 22)) { atomicOr(P.err, 1); break; } }
 }
 
 #ifdef B200_K6_PROF
@@ -548,44 +546,37 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
   const int ctuSize = 1 << P.ctuLog2;
   for (;;) {
     __syncthreads();
-    if (tid == 0) { sCtu = atomicAdd(&counters[1], 1); sNext = 0; }
+    if (tid == 0) { sCtu = atomicAdd(&counters[1], 1); sNext = V2_GROUPS; }
     __syncthreads();
     if (sCtu >= counters[0] || (*(volatile int*)P.err & 2)) return;          // bit 2: a CTU's blocks are not contiguous in the list (intra_ctu_check_kernel)
     const int ctu = ctuOrder[sCtu], first = P.ctuFirst[ctu], cnt = P.ctuCnt[ctu];
     long long tp = clock64(); (void)tp;
-    V2Tile TL;
-    {
-      const int cx = (ctu % P.ctusW) << P.ctuLog2, cy = (ctu / P.ctusW) << P.ctuLog2;
-      int16_t* r = tileRec; int16_t* q = tileRes;
-      for (int c = 0; c < 3; c++) {
-        const int sh = c ? 1 : 0;
-        TL.ox[c] = cx >> sh; TL.oy[c] = cy >> sh; TL.tw[c] = min(ctuSize, P.W - cx) >> sh; TL.th[c] = min(ctuSize, P.H - cy) >> sh; TL.ts[c] = c ? V2_CS : V2_LS;
-        TL.rec[c] = r; TL.res[c] = q; TL.plane[c] = P.planes[c]; TL.ps[c] = P.stride[c];
-        r += (c ? 64 * V2_CS : 128 * V2_LS); q += (c ? 64 * V2_CS : 128 * V2_LS);
-        if (c >= nComp) { TL.tw[c] = TL.th[c] = 0; }
-      }
-    }
+    // the CTU's luma origin and extent; component c's tile is these >> (c ? 1 : 0), at v2_tile_off(c) in the tile sets (plain values, not arrays indexed by
+    // the block's component: such an array would live in local memory)
+    const int cx = (ctu % P.ctusW) << P.ctuLog2, cy = (ctu / P.ctusW) << P.ctuLog2, cw = min(ctuSize, P.W - cx), ch = min(ctuSize, P.H - cy);
     // ---- the CTU's samples, residuals and owner words -> shared memory (asynchronous 32-bit copies: the pitch is not a multiple of 16 bytes), records, flags
     for (int c = 0; c < nComp; c++) {
-      const int16_t* src = P.planes[c] + (size_t)TL.oy[c] * P.stride[c] + TL.ox[c];
-      const int16_t* rsrc = P.resi[c] ? P.resi[c] + (size_t)TL.oy[c] * P.stride[c] + TL.ox[c] : nullptr;
-      if (!(P.stride[c] & 7) && !(TL.tw[c] & 7) && !((uintptr_t)src & 15) && !((uintptr_t)rsrc & 15)) {       // rows start on 16-byte boundaries: 8 samples per copy
-        const int wv = TL.tw[c] >> 3, n = wv * TL.th[c];
+      const int sh = c ? 1 : 0, ox = cx >> sh, oy = cy >> sh, tw = cw >> sh, th = ch >> sh, ts = c ? V2_CS : V2_LS;
+      int16_t* rec = tileRec + v2_tile_off(c); int16_t* res = tileRes + v2_tile_off(c);
+      const int16_t* src = P.planes[c] + (size_t)oy * P.stride[c] + ox;
+      const int16_t* rsrc = P.resi[c] ? P.resi[c] + (size_t)oy * P.stride[c] + ox : nullptr;
+      if (!(P.stride[c] & 7) && !(tw & 7) && !((uintptr_t)src & 15) && !((uintptr_t)rsrc & 15)) {       // rows start on 16-byte boundaries: 8 samples per copy
+        const int wv = tw >> 3, n = wv * th;
         for (int k = tid; k < n; k += V2_THREADS) {
           const int y = k / wv, x = (k - y * wv) * 8;
-          v2_cp16(TL.rec[c] + y * TL.ts[c] + x, src + (size_t)y * P.stride[c] + x);
-          if (rsrc) v2_cp16(TL.res[c] + y * TL.ts[c] + x, rsrc + (size_t)y * P.stride[c] + x);
+          v2_cp16(rec + y * ts + x, src + (size_t)y * P.stride[c] + x);
+          if (rsrc) v2_cp16(res + y * ts + x, rsrc + (size_t)y * P.stride[c] + x);
         }
       } else {
-        const int wWords = TL.tw[c] >> 1, n = wWords * TL.th[c];
+        const int wWords = tw >> 1, n = wWords * th;
         for (int k = tid; k < n; k += V2_THREADS) {
           const int y = k / wWords, x = (k - y * wWords) * 2;
-          v2_cp4(TL.rec[c] + y * TL.ts[c] + x, src + (size_t)y * P.stride[c] + x);
-          if (rsrc) v2_cp4(TL.res[c] + y * TL.ts[c] + x, rsrc + (size_t)y * P.stride[c] + x);
+          v2_cp4(rec + y * ts + x, src + (size_t)y * P.stride[c] + x);
+          if (rsrc) v2_cp4(res + y * ts + x, rsrc + (size_t)y * P.stride[c] + x);
         }
       }
-      const int unit = c ? 2 : 4, uw = TL.tw[c] / unit, uh = TL.th[c] / unit;
-      const int* osrc = P.owner[c] + (size_t)(TL.oy[c] / unit) * P.ownerStride[c] + TL.ox[c] / unit;
+      const int unit = c ? 2 : 4, uw = tw / unit, uh = th / unit;
+      const int* osrc = P.owner[c] + (size_t)(oy / unit) * P.ownerStride[c] + ox / unit;
       for (int k = tid; k < uw * uh; k += V2_THREADS) { const int y = k / uw, x = k - y * uw; v2_cp4(sown + c * 1024 + y * 32 + x, osrc + (size_t)y * P.ownerStride[c] + x); }
     }
     for (int k = tid; k < min(cnt, V2_RECS) * 4; k += V2_THREADS) v2_cp4(reinterpret_cast<uint32_t*>(srec) + k, reinterpret_cast<const uint32_t*>(P.tus + first) + k);
@@ -597,29 +588,28 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
     // ---- the CTU's blocks, one group each, in decoding order
     V2Scratch& SC = scratch[grp];
 #define V2_SYNC() do { if (V2_GROUP == 32) __syncwarp(); else asm volatile("bar.sync %0, %1;" :: "r"(grp + 1), "r"(V2_GROUP) : "memory"); } while (0)
-    for (;;) {
-      V2_SYNC();
-      if (lane == 0) { SC.ticket = atomicAdd(&sNext, 1); SC.sum = 0; }
-      V2_SYNC();
-      const int k = SC.ticket;
-      if (k >= cnt) break;
+    // Block tickets: group g starts with block g (sNext starts past them); while a group works on a block, its lane 0 takes the group's next ticket.  Tickets
+    // still go out in decoding order and only to running groups.  The ticket alternates between two words: between lane 0's write of a word and the group's
+    // read of it lies the block's last barrier, and between that read and lane 0's next write of the same word the next block's first barrier.
+    int slot = 0;
+    for (int k = grp; k < cnt; k = SC.next[slot], slot ^= 1) {
+      if (lane == 0) { SC.next[slot] = atomicAdd(&sNext, 1); SC.sum = 0; }
       tp = clock64(); const long long tb0 = tp; (void)tb0;
       const int me = first + k;
       const b200_intra_tu t = k < V2_RECS ? srec[k] : P.tus[me];
-      if ((P.compSel == 1 && t.comp != 0) || (P.compSel == 2 && t.comp == 0)) continue;      // the other channel's pass
+      if ((P.compSel == 1 && t.comp != 0) || (P.compSel == 2 && t.comp == 0)) { V2_SYNC(); continue; }      // the other channel's pass
       const int c = t.comp, w = 1 << t.log2w, h = 1 << t.log2h, mrl = c ? 0 : t.multiRefIdx, unit = c ? 2 : 4;
       const int x0 = t.x, y0 = t.y, ps = P.stride[c], pmax = (1 << P.bitDepth) - 1;
       const int availTL = (t.flags & B200_INTRA_AVAIL_TL) ? 1 : 0, numAbove = t.numAbove, numLeft = t.numLeft;
       ISP_GEOMETRY
-      // the tile of the block's component, in registers (indexing the per-component arrays with a run-time index would go through local memory)
-      const int tox = TL.ox[c], toy = TL.oy[c], ttw = TL.tw[c], tth = TL.th[c], tts = TL.ts[c];
-      const int16_t* trec = TL.rec[c]; const int16_t* tplane = TL.plane[c];
+      // the tile of the block's component
+      const int csh = c ? 1 : 0, tox = cx >> csh, toy = cy >> csh, ttw = cw >> csh, tth = ch >> csh, tts = c ? V2_CS : V2_LS;
+      int16_t* trec = tileRec + v2_tile_off(c); const int16_t* tplane = P.planes[c];
       auto pixC = [&](int x, int y) -> int {
         return ((unsigned)(x - tox) < (unsigned)ttw && (unsigned)(y - toy) < (unsigned)tth) ? (int)trec[(y - toy) * tts + (x - tox)] : (int)__ldcg(tplane + (size_t)y * ps + x);
       };
       // ---- wait for the earlier blocks this one reads from
-      bool far = false;
-      if (ispK && lane == 0) far |= v2_wait(P, sflag, me - 1, me, first);     // ISP: the region before this one is the record before it
+      if (ispK && lane == 0) v2_wait(P, sflag, me - 1, me, first);          // ISP: the region before this one is the record before it
       for (int dep = lane; dep < 96; dep += V2_GROUP) {                        // dependency slots: 0 corner, 1..32 above units, 64..95 left units
         int ux = -1, uy = -1;
         if (dep == 0) { if (availTL) { ux = bx - 1; uy = by - 1; } }
@@ -628,7 +618,7 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
         if (ux >= 0 && uy >= 0) {
           const int ush = c ? 1 : 2, ox = (ux >> ush) - (tox >> ush), oy = (uy >> ush) - (toy >> ush);          // inside the CTU: the staged owner word
           const int o = ((unsigned)ox < 32u && (unsigned)oy < 32u && ux < tox + ttw && uy < toy + tth) ? sown[c * 1024 + oy * 32 + ox] : __ldcg(P.owner[c] + (size_t)(uy >> ush) * P.ownerStride[c] + (ux >> ush));
-          far |= v2_wait(P, sflag, o, me, first);
+          v2_wait(P, sflag, o, me, first);
         }
       }
       if (t.mode >= B200_INTRA_LM) {
@@ -638,12 +628,11 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
         const int uy0 = max(0, (2 * y0 - (aCu ? 4 : 0)) >> 2), uy1 = min(P.H - 1, 2 * y0 + 2 * nL - 1) >> 2;
         const int uw = ux1 - ux0 + 1, nU = uw * (uy1 - uy0 + 1);
         for (int u = lane; u < nU; u += V2_GROUP) {
-          const int gx = ux0 + u % uw, gy = uy0 + u / uw, ox = gx - TL.ox[0] / 4, oy = gy - TL.oy[0] / 4;
-          const int o = ((unsigned)ox < 32u && (unsigned)oy < 32u && gx * 4 < TL.ox[0] + TL.tw[0] && gy * 4 < TL.oy[0] + TL.th[0]) ? sown[oy * 32 + ox] : __ldcg(P.owner[0] + (size_t)gy * P.ownerStride[0] + gx);
-          far |= v2_wait(P, sflag, o, me, first);
+          const int gx = ux0 + u % uw, gy = uy0 + u / uw, ox = gx - cx / 4, oy = gy - cy / 4;
+          const int o = ((unsigned)ox < 32u && (unsigned)oy < 32u && gx * 4 < cx + cw && gy * 4 < cy + ch) ? sown[oy * 32 + ox] : __ldcg(P.owner[0] + (size_t)gy * P.ownerStride[0] + gx);
+          v2_wait(P, sflag, o, me, first);
         }
       }
-      if (far) __threadfence(); else __threadfence_block();      // a thread that saw another CTU's done word orders the plane reads of its group behind it
       V2_SYNC();
       const int pb = c ? 16 : 0; (void)pb;
       K6P(pb + 1, tp); tp = clock64();                          // [1] dependency wait
@@ -656,12 +645,22 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
 #define PIXR(x, y) pixC((x), (y))
       ISP_REFERENCE_LAMBDAS
       // one pass over both arrays: a thread takes entry j of the row and entry j of the column (two independent fetches in flight); entry 0 of the column is the corner
-      for (int j = lane; j <= max(topLen, sideLen) + mrl; j += V2_GROUP) {
-        const bool doT = j <= topLen + mrl, doL = j >= 1 && j <= sideLen + mrl;
-        const int vt = doT ? regT(j) : 0, vl = doL ? regL(j) : 0;
-        if (doT) T[j] = (int16_t)vt;
-        if (doL) L[j] = (int16_t)vl;
-        if (j == 0) L[0] = (int16_t)vt;
+      if (!isp && n == totalUnits) {                             // the whole neighbourhood is available (most blocks): straight copies
+        const int rx = bx - 1 - mrl, ry = by - 1 - mrl;
+        for (int j = lane; j <= max(topLen, sideLen) + mrl; j += V2_GROUP) {
+          const bool doT = j <= topLen + mrl, doL = j <= sideLen + mrl;
+          const int vt = doT ? pixC(rx + j, ry) : 0, vl = doL ? pixC(rx, ry + j) : 0;
+          if (doT) T[j] = (int16_t)vt;
+          if (doL) L[j] = (int16_t)vl;
+        }
+      } else {
+        for (int j = lane; j <= max(topLen, sideLen) + mrl; j += V2_GROUP) {
+          const bool doT = j <= topLen + mrl, doL = j >= 1 && j <= sideLen + mrl;
+          const int vt = doT ? regT(j) : 0, vl = doL ? regL(j) : 0;
+          if (doT) T[j] = (int16_t)vt;
+          if (doL) L[j] = (int16_t)vl;
+          if (j == 0) L[0] = (int16_t)vt;
+        }
       }
 #undef PIXR
       V2_SYNC();
@@ -681,9 +680,9 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
       const int mode = t.mode;
       const bool doPDPC = w >= 4 && h >= 4 && mrl == 0;
       int16_t* dstG = P.planes[c] + (size_t)y0 * ps + x0;
-      int16_t* dstT = const_cast<int16_t*>(trec) + (y0 - toy) * tts + (x0 - tox);
+      int16_t* dstT = trec + (y0 - toy) * tts + (x0 - tox);
       const int tsC = tts;
-      const int16_t* rsT = (P.resi[c] && (t.flags & B200_INTRA_ADD_RESI)) ? TL.res[c] + (y0 - toy) * tsC + (x0 - tox) : nullptr;
+      const int16_t* rsT = (P.resi[c] && (t.flags & B200_INTRA_ADD_RESI)) ? tileRes + v2_tile_off(c) + (y0 - toy) * tsC + (x0 - tox) : nullptr;
       const int ciipW = isp ? 0 : t.ciip;
 #define V2_STORE(x, y, v) do { int v_ = (v); int16_t* d_ = dstT + (y) * tsC + (x); if (ciipW) v_ = ((4 - ciipW) * (int)*d_ + ciipW * v_ + 2) >> 2; \
                                if (rsT && ((resiMask >> ((x) >> l2tu)) & 1)) v_ = clip3(0, pmax, v_ + rsT[(y) * tsC + (x)]); *d_ = (int16_t)v_; dstG[(size_t)(y) * ps + (x)] = (int16_t)v_; } while (0)
@@ -725,9 +724,9 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
         const int lx0 = 2 * x0, ly0 = 2 * y0;
         const bool firstRowOfCtu = ((2 * y0) & ((1 << P.ctuLog2) - 1)) == 0;
         const int nTop = aCu ? (mode == B200_INTRA_MDLM_T ? 2 * t.lmAbove : w) : 0, nLeft = lCu ? (mode == B200_INTRA_MDLM_L ? 2 * t.lmLeft : h) : 0;
-        const int lox = TL.ox[0], loy = TL.oy[0], ltw = TL.tw[0], lth = TL.th[0]; const int16_t* lrec = TL.rec[0]; const int16_t* lplane = TL.plane[0]; const int lps = TL.ps[0];
+        const int16_t* lplane = P.planes[0]; const int lps = P.stride[0];
         auto pixY = [&](int x, int y) -> int {
-          return ((unsigned)(x - lox) < (unsigned)ltw && (unsigned)(y - loy) < (unsigned)lth) ? (int)lrec[(y - loy) * V2_LS + (x - lox)] : (int)__ldcg(lplane + (size_t)y * lps + x);
+          return ((unsigned)(x - cx) < (unsigned)cw && (unsigned)(y - cy) < (unsigned)ch) ? (int)tileRec[(y - cy) * V2_LS + (x - cx)] : (int)__ldcg(lplane + (size_t)y * lps + x);
         };
 #define LY(dx, dy) pixY(lx0 + (dx), ly0 + (dy))
         for (int kk = lane; kk < nTop + nLeft + w * h; kk += V2_GROUP) {
@@ -846,17 +845,17 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
         const int invAngle = cInvAng[absMode], absAng = cAng[absMode], angle = angMode < 0 ? -absAng : absAng;
         const int16_t *mainSrc = ver ? T : L, *sideSrc = ver ? L : T;
         const int mw = ver ? w : h, mh = ver ? h : w;
-        int16_t *M = SC.M + IT_ORG, *S = SC.S + IT_ORG;
+        // angles >= 0 read the main reference directly, clamped to its end (the replication tail of xPredIntraAng); negative angles stage the main array
+        // with the side reference projected in front of it.  Only angles >= 0 read the side reference.
+        const int16_t *Mp, *Sp = sideSrc + mrl;
+        int mEnd;                                                  // last main index read as is: later ones read entry mEnd
         if (angle < 0) {
+          int16_t* M = SC.M + IT_ORG;
           for (int kk = lane - mh; kk <= mw + 1 + mrl; kk += V2_GROUP) M[kk] = kk >= 0 ? mainSrc[kk] : sideSrc[min((-kk * invAngle + 256) >> 9, mh)];
-          for (int kk = lane; kk <= mh + 1 + mrl; kk += V2_GROUP) S[kk] = sideSrc[kk];
-        } else {
-          const int l2r = (31 - __clz(mw)) - (31 - __clz(mh)), sft = max(0, l2r), maxIndex = (mrl << sft) + 2, refLength = ver ? topLen : sideLen;
-          for (int kk = lane; kk <= refLength + mrl + maxIndex; kk += V2_GROUP) M[kk] = mainSrc[min(kk, refLength + mrl)];
-          for (int kk = lane; kk <= (ver ? sideLen : topLen) + mrl; kk += V2_GROUP) S[kk] = sideSrc[kk];
-        }
-        V2_SYNC();
-        const int16_t *Mp = M + mrl, *Sp = S + mrl;
+          V2_SYNC();
+          Mp = M + mrl; mEnd = 1 << 20;
+        } else { Mp = mainSrc + mrl; mEnd = ver ? topLen : sideLen; }
+#define MAIN(i) Mp[min((i), mEnd)]
         const int l2mw = 31 - __clz(mw), l2mh = 31 - __clz(mh);
         const int topLeft = T[0];
         const int scale0 = (l2mw - 2 + l2mh - 2 + 2) >> 2;
@@ -871,18 +870,18 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
           const int yy = kk >> l2mw, xx = kk & (mw - 1);
           int v;
           if (angle == 0) {
-            if (doPDPC && xx < lev) { const int wL = 32 >> min(31, (xx << 1) >> scale0); v = clip3(0, pmax, (wL * (Sp[yy + 1] - topLeft) + Mp[xx + 1] * 64 + 32) >> 6); }
-            else v = Mp[xx + 1];
+            if (doPDPC && xx < lev) { const int wL = 32 >> min(31, (xx << 1) >> scale0); v = clip3(0, pmax, (wL * (Sp[yy + 1] - topLeft) + MAIN(xx + 1) * 64 + 32) >> 6); }
+            else v = MAIN(xx + 1);
           } else {
             const int deltaPos = angle * (1 + mrl + yy), dI = deltaPos >> 5, dF = deltaPos & 31;
-            if (!frac) v = Mp[dI + 1 + xx];
-            else if (c) v = (int16_t)(((32 - dF) * Mp[dI + 1 + xx] + dF * Mp[dI + 2 + xx] + 16) >> 5);
+            if (!frac) v = MAIN(dI + 1 + xx);
+            else if (c) v = (int16_t)(((32 - dF) * MAIN(dI + 1 + xx) + dF * MAIN(dI + 2 + xx) + 16) >> 5);
             else {
-              const int16_t* p = Mp + dI + xx;
+              const int p = dI + xx;
               int f0, f1, f2, f3;
               if (cubic) { f0 = kIfChroma[dF * 4]; f1 = kIfChroma[dF * 4 + 1]; f2 = kIfChroma[dF * 4 + 2]; f3 = kIfChroma[dF * 4 + 3]; }
               else { f0 = 16 - (dF >> 1); f1 = 32 - (dF >> 1); f2 = 16 + (dF >> 1); f3 = dF >> 1; }
-              v = (int16_t)((f0 * p[0] + f1 * p[1] + f2 * p[2] + f3 * p[3] + 32) >> 6);
+              v = (int16_t)((f0 * MAIN(p) + f1 * MAIN(p + 1) + f2 * MAIN(p + 2) + f3 * MAIN(p + 3) + 32) >> 6);
               if (cubic) v = clip3(0, pmax, v);
             }
             if (angularScale >= 0 && xx < min(3 << angularScale, mw)) {
@@ -892,18 +891,18 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
           }
           if (ver) V2_STORE(xx, yy, v); else V2_STORE(yy, xx, v);
         }
+#undef MAIN
       }
 #undef V2_STORE
       // ---- publish: the CTU's own later blocks see the tile; other CTUs read the plane, and only the samples of the CTU's last column and last row
-      // (left, above and above-right references of the CTUs right of / below it): blocks that touch neither skip the device-scope fence and the done word
-      __threadfence_block();
+      // (left, above and above-right references of the CTUs right of / below it): blocks that touch neither skip the done word.  After the group barrier
+      // one thread releases the group's stores: at CTA scope through the done byte, at GPU scope through the done word (both cumulative over the barrier)
       V2_SYNC();
       K6P(pb + 3, tp); tp = clock64();                          // [3] prediction + stores
-      if (lane == 0) sflag[k] = 1;
-      if (x0 + w == tox + ttw || y0 + h == toy + tth) {
-        __threadfence();
-        V2_SYNC();
-        if (lane == 0) atomicExch(P.done + me, 1);
+      if (lane == 0) {
+        __threadfence_block();
+        sflag[k] = 1;
+        if (x0 + w == tox + ttw || y0 + h == toy + tth) v2_st_release(P.done + me, 1);
       }
       K6P(pb + 4, tp); K6C(pb + 9); K6P(pb + 10 + min(4, max(0, ((int)t.log2w + (int)t.log2h - 4) >> 1)), tb0);   // [4] device fence + done word, [9] blocks, [10..14] whole block by size class
     }
@@ -975,6 +974,10 @@ int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_ge
   return 0;
 }
 
+// CTU-resident grid: CTAs per CTU of the widest wave-front diagonal, times 2.  Single-lane 4K I picture on an H100 80 GB HBM3 at 400 W, 128x5 groups
+// (bench.py --lanes 1, I_picture_ms): 1x 10.15 ms, 1.5x 9.64, 2x 9.56, 3x 9.43, SM count (132 CTAs) 9.42 — 3x is the smallest factor that costs nothing
+constexpr int kWaveCtasPerDiag2 = 6;
+
 int launch_intra(const IntraLaunch& L, cudaStream_t s)
 {
   if (!L.numTus) return 0;
@@ -1010,12 +1013,23 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
       intra_ctu_check_kernel<<<grid, 256, 0, s>>>(P);
       intra_ctu_order_kernel<<<1, 1024, nCtu * sizeof(int), s>>>(P, ctuOrder, counters);
     }
-    const int ctas = (int)std::min<size_t>(nCtu, (size_t)num_sms());
+    // Grid: as many CTAs as the wave front can keep busy.  Only the CTUs of about one key x + 2 y (at most `diag` of them) run at a time — with the next
+    // key's CTUs trailing them by a fraction of a CTU — and each CTA fills an SM (registers and shared memory), so a grid of SM count would hold SMs that
+    // spin on done words, away from the other work of the device (the second lane's picture).  Any grid of at least one CTA is deadlock-free: CTU tickets
+    // go out in wave-front order and only to running CTAs, so the oldest unfinished CTU never waits on one that has not started.
+    int diag = 1;
+    for (int key = 0; key < P.ctusW + 2 * P.ctusH; key++) {
+      int n = 0;
+      for (int y = 0; y < P.ctusH; y++) n += key - 2 * y >= 0 && key - 2 * y < P.ctusW;
+      diag = std::max(diag, n);
+    }
+    const int ctas = (int)std::min<size_t>({nCtu, (size_t)num_sms(), (size_t)(kWaveCtasPerDiag2 * diag + 1) / 2});
     static const int shape = getenv("B200_INTRA_GROUP") ? atoi(getenv("B200_INTRA_GROUP")) : 0;      // measurement switch: threads per block group
 #define V2_GO(G, N) do { static bool attr = false; if (!attr) { B200_CUDA(cudaFuncSetAttribute(intra_ctu_kernel<G, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)v2_smem(N))); attr = true; } \
                          intra_ctu_kernel<G, N><<<ctas, G * N, v2_smem(N), s>>>(P, ctuOrder, counters); } while (0)
-    // measured on a 4K I picture (66810 blocks): 128x4 7.45 ms, 128x6 6.97 ms, 128x8 7.70 ms, 64x6 7.62 ms, 64x12 7.61 ms, 256x3 9.22 ms, 32x8 17.9 ms
-    if (shape == 1284) V2_GO(128, 4); else if (shape == 32) V2_GO(32, 8); else V2_GO(128, 6);
+    // 128x5: 96 registers, no spills (128x6 is capped at 80 and spills).  Single-lane 4K I picture, grid 2x the diagonal, H100 80 GB HBM3 at 400 W:
+    // 128x5 9.56 ms, 128x6 9.99 ms
+    if (shape == 1284) V2_GO(128, 4); else if (shape == 32) V2_GO(32, 8); else V2_GO(128, 5);
 #undef V2_GO
     B200_CUDA(cudaGetLastError());
     return 0;
