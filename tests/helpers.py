@@ -1,5 +1,5 @@
 """Test helpers: load the oracle (C restatement) and, when built, the reference shim."""
-import os, subprocess, ctypes as C
+import contextlib, os, subprocess, ctypes as C
 import numpy as np
 from vvdec_b200 import abi, synth
 
@@ -424,3 +424,91 @@ def intra_picture_case(ref, rng, W, H, bd, ctu, simd, p_resi=0.5, colloc=0, **la
     n = ref.ref_intra_case(simd, C.byref(g), abi.plane_ptrs(out), abi.plane_ptrs(resi), cus.ctypes.data, len(layout), 1, recs.ctypes.data, len(recs), colloc)
     assert n > 0, n
     return g, planes, resi, recs[:n], out
+
+
+# ---- K6 kernel choice: launch_intra reads B200_INTRA_KERNEL / B200_INTRA_ORDER on every launch
+INTRA_KERNELS = ("auto", "v1", "v1_decode", "v2")
+_INTRA_ENV = {"auto": {}, "v1": {"B200_INTRA_KERNEL": "v1"}, "v1_decode": {"B200_INTRA_KERNEL": "v1", "B200_INTRA_ORDER": "decode"}, "v2": {"B200_INTRA_KERNEL": "v2"}}
+
+
+@contextlib.contextmanager
+def intra_kernel(kernel):
+    """While the block runs, K6 takes `kernel`: auto (chosen by list density), v1 (one CTA per block; wave-front tickets for dense lists, list order
+    otherwise), v1_decode (v1, tickets in list order), v2 (CTU-resident; v1 where a plane stride is odd)."""
+    keys = ("B200_INTRA_KERNEL", "B200_INTRA_ORDER")
+    old = {k: os.environ.get(k) for k in keys}
+    for k in keys: os.environ.pop(k, None)
+    os.environ.update(_INTRA_ENV[kernel])
+    try:
+        yield
+    finally:
+        for k, v in old.items():
+            if v is None: os.environ.pop(k, None)
+            else: os.environ[k] = v
+
+
+def intra_run(b200, kernel, g, planes, recs, resi=None):
+    """b200_intra_reconstruct (b200_intra_predict without residual planes) of `recs` on copies of `planes` under `kernel`; returns the planes."""
+    import vvdec_b200
+    got = [None if p is None else p.copy() for p in planes]
+    with intra_kernel(kernel):
+        if resi is None: vvdec_b200.check(b200.b200_intra_predict(C.byref(g), abi.plane_ptrs(got), recs.ctypes.data, len(recs)))
+        else: vvdec_b200.check(b200.b200_intra_reconstruct(C.byref(g), abi.plane_ptrs(got), abi.plane_ptrs(resi), recs.ctypes.data, len(recs)))
+    return got
+
+
+def assert_planes_equal(got, want, what=""):
+    """Bit-exact planes; a failure names the plane, the number of differing samples and the first four (y, x)."""
+    for c, (a, b) in enumerate(zip(got, want)):
+        if b is None: continue
+        bad = np.argwhere(a != b)
+        assert len(bad) == 0, (what, c, len(bad), bad[:4].tolist())
+
+
+def intra_dense(g, n):
+    """launch_intra's density rule: at least 48 records per 128x128 luma area picks the CTU-resident kernel under auto."""
+    return n >= 48 * max(1, (g.width * g.height) >> 14)
+
+
+def intra_ctu_counts(recs, ctu, W):
+    """Records per CTU (chroma positions scaled to luma)."""
+    sh = (recs["comp"] > 0).astype(np.int64)
+    cw = (W + ctu - 1) // ctu
+    return np.bincount(((recs["y"].astype(np.int64) << sh) // ctu) * cw + ((recs["x"].astype(np.int64) << sh) // ctu))
+
+
+# K6 cases beyond the random all-intra pictures: geometry, formats, bit depths and capacity (name -> keyword arguments of intra_case)
+INTRA_CASES = {
+    "ctu32_256x128": dict(W=256, H=128, ctu=32, min_size=4, p_isp=0.3, seed=21),
+    "ctu32_416x240": dict(W=416, H=240, ctu=32, min_size=4, p_isp=0.3, seed=22),
+    "ctu64_200x136": dict(W=200, H=136, ctu=64, min_size=4, p_isp=0.3, seed=23),            # partial CTUs: 8 x 8 luma corner, 4-wide / 4-high chroma tiles
+    "stride_420": dict(W=416, H=240, ctu=128, min_size=4, strides=(420, 210, 210), seed=24),   # even strides, not a multiple of 8 samples
+    "stride_417": dict(W=416, H=240, ctu=128, min_size=4, strides=(417, 209, 209), seed=25),   # odd stride: v1 under every setting
+    "yuv400_8bit": dict(W=256, H=128, ctu=128, min_size=4, bd=8, chroma=False, seed=26),
+    "yuv400_12bit": dict(W=256, H=128, ctu=128, min_size=4, bd=12, chroma=False, seed=27),
+    "8bit_832x480": dict(W=832, H=480, ctu=128, min_size=4, bd=8, p_mip=0.4, seed=28),
+    "12bit_832x480": dict(W=832, H=480, ctu=128, min_size=4, bd=12, p_mip=0.4, seed=29),
+    "ctu_1244_blocks": dict(W=256, H=128, ctu=128, min_size=8, p_split=1.0, p_isp=0.9, p_mip=0.0, p_mrl=0.0, p_bdpcm=0.0, p_lm=0.0, seed=7),
+    "ctu_1024_blocks": dict(W=256, H=128, ctu=128, min_size=4, p_split=1.0, p_isp=0.9, p_mip=0.0, p_mrl=0.0, p_bdpcm=0.0, p_lm=0.0, seed=7),
+    "sparse_1080p": dict(W=1920, H=1080, ctu=128, min_size=8, p_split=0.6, intra=0.15, p_ciip=0.1, seed=30),   # the intra / CIIP blocks of a B picture
+}
+
+
+def intra_case(W, H, ctu, seed, min_size=8, bd=10, chroma=True, strides=None, p_split=0.75, p_isp=0.0, p_mip=0.15, p_mrl=0.15, p_bdpcm=0.08, p_lm=0.25, intra=None, p_ciip=0.25):
+    """A list of gen_intra_records on noise planes with residual planes: returns (geometry, planes, residual planes, records).  intra: fraction of
+    intra CUs (the others are inter CUs, p_ciip of those with a CIIP block of weight 1..3); None: every CU is intra."""
+    rng = np.random.default_rng(seed)
+    g = abi.make_geom(W, H, bd, chroma_format=1 if chroma else 0, ctu=ctu, strides=strides)
+    layout = synth.gen_intra_layout(rng, W, H, ctu, min_size=min_size, p_split=p_split)
+    only, ciip = None, None
+    if intra is not None:
+        only = rng.random(len(layout)) < intra
+        ciip = {i: int(rng.integers(1, 4)) for i, (x, y, w, h) in enumerate(layout) if not only[i] and w * h >= 64 and rng.random() < p_ciip}
+        for i in ciip: only[i] = True
+    recs = synth.gen_intra_records(rng, layout, W, H, p_resi=0.5, p_lm=p_lm if chroma else 0.0, p_isp=p_isp, p_mip=p_mip, p_mrl=p_mrl, p_bdpcm=p_bdpcm,
+                                   colloc=seed & 1, only=only, ciip=ciip, ctu=ctu)
+    if not chroma: recs = np.ascontiguousarray(recs[recs["comp"] == 0])
+    planes = synth.noise_planes(rng, W, H, bd, chroma=chroma, strides=strides)
+    resi = [rng.integers(-40, 41, size=p.shape).astype(np.int16) for p in planes]
+    if not chroma: planes, resi = planes + [None, None], resi + [None, None]
+    return g, planes, resi, recs

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import vvdec_b200
 from vvdec_b200 import abi, synth
-from tests.helpers import oracle_decompress
+from tests.helpers import oracle_decompress, intra_kernel
 
 pytestmark = pytest.mark.gpu
 
@@ -117,7 +117,18 @@ def test_invalid_records_are_reported(b200):
 def test_lmcs_picture(b200, oracle, W, H, ctu, chroma_adj):
     """LMCS on (SURVEY 8 row a17): forward-mapped luma prediction fused into K2, luma TUs -> per-VPDU chroma scale -> scaled chroma
     TUs, inverse map before deblocking — against the oracle chain (which tests/test_lmcs_oracle_vs_ref.py pins to the real Reshape)."""
-    rng = np.random.default_rng(W + ctu)
+    _lmcs_pictures(b200, oracle, W, H, ctu, chroma_adj, 0.0, ["auto"])
+
+
+@pytest.mark.parametrize("W,H,ctu,intra_frac", [(416, 240, 128, 0.15), (416, 240, 64, 1.0)])
+def test_lmcs_picture_with_intra_cus(b200, oracle, W, H, ctu, intra_frac):
+    """LMCS with intra and CIIP CUs: K6 runs twice on one list (luma blocks, then after the VPDU scales the chroma blocks, the luma blocks marked
+    done), every picture under each kernel."""
+    _lmcs_pictures(b200, oracle, W, H, ctu, True, intra_frac, ["v1", "v2"])
+
+
+def _lmcs_pictures(b200, oracle, W, H, ctu, chroma_adj, intra_frac, kernels):
+    rng = np.random.default_rng(W + ctu + int(100 * intra_frac))
     bd = 10
     g = abi.make_geom(W, H, bd, ctu=ctu)
     ctx = C.c_void_p()
@@ -126,17 +137,19 @@ def test_lmcs_picture(b200, oracle, W, H, ctu, chroma_adj):
         dpb = [synth.noise_planes(rng, W, H, bd) for _ in range(4)]
         for s in range(4): vvdec_b200.check(b200.b200_ctx_load_slot(ctx, s, abi.plane_ptrs(dpb[s])))
         for k in range(2):
-            pic = synth.gen_picture(rng, W, H, bd, ctu=ctu, dst_slot=4 + k, lmcs=True, lmcs_chroma=chroma_adj)
+            pic = synth.gen_picture(rng, W, H, bd, ctu=ctu, dst_slot=4 + k, lmcs=True, lmcs_chroma=chroma_adj, intra_frac=intra_frac)
+            if intra_frac: assert len(pic["intraTus"]) and (pic["intraTus"]["comp"] > 0).any()
             want, dm_want = oracle_decompress(oracle, g, dpb, pic)
-            h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"]))
-            assert h >= 0, b200.b200_last_error()
-            dm = np.zeros((pic["ndmvr"] + 1, 2), np.int32)
-            vvdec_b200.check(b200.b200_wait_picture(ctx, h, dm.ctypes.data, len(dm)))
-            got = [np.zeros_like(p) for p in want]
-            vvdec_b200.check(b200.b200_get_frame(ctx, 4 + k, abi.plane_ptrs(got)))
-            for c in range(3):
-                assert np.array_equal(want[c], got[c]), f"picture {k} plane {c}: {len(np.argwhere(want[c] != got[c]))} diffs"
-            assert np.array_equal(dm, dm_want)
+            for kernel in kernels:
+                with intra_kernel(kernel): h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"]))
+                assert h >= 0, b200.b200_last_error()
+                dm = np.zeros((pic["ndmvr"] + 1, 2), np.int32)
+                vvdec_b200.check(b200.b200_wait_picture(ctx, h, dm.ctypes.data, len(dm)))
+                got = [np.zeros_like(p) for p in want]
+                vvdec_b200.check(b200.b200_get_frame(ctx, 4 + k, abi.plane_ptrs(got)))
+                for c in range(3):
+                    assert np.array_equal(want[c], got[c]), f"{kernel}: picture {k} plane {c}: {len(np.argwhere(want[c] != got[c]))} diffs"
+                assert np.array_equal(dm, dm_want)
     finally:
         b200.b200_ctx_destroy(ctx)
 
@@ -164,11 +177,11 @@ def test_weighted_prediction_picture(b200, oracle):
         b200.b200_ctx_destroy(ctx)
 
 
-@pytest.mark.parametrize("W,H,ctu,intra_frac,seed", [(416, 240, 128, 0.25, 1), (416, 240, 64, 1.0, 2), (832, 480, 128, 0.15, 3), (1920, 1080, 128, 0.3, 4)])
+@pytest.mark.parametrize("W,H,ctu,intra_frac,seed", [(416, 240, 128, 0.25, 1), (416, 240, 64, 1.0, 2), (832, 480, 128, 0.15, 3), (1920, 1080, 128, 0.3, 4), (416, 240, 32, 1.0, 5)])
 def test_picture_with_intra_cus(b200, oracle, W, H, ctu, intra_frac, seed):
     """Intra CUs reconstructed on the device inside the picture chain (SURVEY 8f-1, regular modes): K2 for the inter CUs, K1 (inter TUs reconstruct, TUs
     of intra CUs leave their residual in the residual planes), K6 over the intra blocks in decoding order — each reads the reconstruction of inter and
-    earlier intra neighbours — then deblocking / SAO / ALF.  intra_frac 1.0 is an I picture."""
+    earlier intra neighbours — then deblocking / SAO / ALF.  intra_frac 1.0 is an I picture.  Every picture is decoded under each K6 kernel in turn."""
     rng = np.random.default_rng(seed)
     bd = 10
     g = abi.make_geom(W, H, bd, ctu=ctu)
@@ -182,14 +195,16 @@ def test_picture_with_intra_cus(b200, oracle, W, H, ctu, intra_frac, seed):
             assert len(pic["intraTus"]) > 0 and (pic["tus"]["flags"] & abi.TU_RESI).any() and (pic["intraTus"]["flags"] & abi.INTRA_ADD_RESI).any()
             assert intra_frac == 1.0 or (pic["intraTus"]["ciip"] > 0).any()          # CIIP CUs among the inter CUs
             want, dm_want = oracle_decompress(oracle, g, dpb, pic)
-            h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"])); assert h >= 0, b200.b200_last_error()
-            dm = np.zeros((pic["ndmvr"] + 1, 2), np.int32)
-            vvdec_b200.check(b200.b200_wait_picture(ctx, h, dm.ctypes.data, len(dm)))
-            got = [np.zeros_like(p) for p in want]
-            vvdec_b200.check(b200.b200_get_frame(ctx, 4 + i, abi.plane_ptrs(got)))
-            for c in range(3):
-                assert np.array_equal(want[c], got[c]), f"picture {i} plane {c}: {len(np.argwhere(want[c] != got[c]))} diffs"
-            assert np.array_equal(dm, dm_want)
+            for kernel in ("v1", "v2"):
+                with intra_kernel(kernel): h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"]))
+                assert h >= 0, b200.b200_last_error()
+                dm = np.zeros((pic["ndmvr"] + 1, 2), np.int32)
+                vvdec_b200.check(b200.b200_wait_picture(ctx, h, dm.ctypes.data, len(dm)))
+                got = [np.zeros_like(p) for p in want]
+                vvdec_b200.check(b200.b200_get_frame(ctx, 4 + i, abi.plane_ptrs(got)))
+                for c in range(3):
+                    assert np.array_equal(want[c], got[c]), f"{kernel}: picture {i} plane {c}: {len(np.argwhere(want[c] != got[c]))} diffs"
+                assert np.array_equal(dm, dm_want)
         # a record whose availability reaches outside the picture is refused
         bad = pic["intraTus"]; keep = bad[0].copy(); bad[0]["numAbove"] = 3; bad[0]["y"] = 0
         assert b200.b200_decompress_picture(ctx, C.byref(pic["struct"])) == -2 and b"intra block record" in b200.b200_last_error()
@@ -222,3 +237,88 @@ def test_failed_host_register_does_not_resurface(b200, oracle):
         for c in range(3): assert np.array_equal(want[c], got[c]), f"plane {c}"
     finally:
         b200.b200_ctx_destroy(ctx); b200.b200_host_unregister(buf.ctypes.data)
+
+
+@pytest.mark.parametrize("kernel", ["auto", "v1", "v2"])
+def test_intra_list_refusals(b200, oracle, kernel):
+    """Intra lists the CTU-resident kernel cannot address are refused, and the context then decodes the next picture: a block that is not inside one
+    CTU (b200_decompress_picture, before anything runs), and more than 3072 blocks in one CTU (overlapping records; only the CTU-resident kernel counts
+    them, so b200_wait_picture reports it and the one-CTA-per-block kernel reconstructs the list)."""
+    rng = np.random.default_rng(41)
+    W, H, bd, ctu = 416, 240, 10, 64
+    g = abi.make_geom(W, H, bd, ctu=ctu)
+    ctx = C.c_void_p()
+    vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 2, -1))
+    try:
+        dpb = [synth.noise_planes(rng, W, H, bd) for _ in range(4)]
+        for s in range(4): vvdec_b200.check(b200.b200_ctx_load_slot(ctx, s, abi.plane_ptrs(dpb[s])))
+        pic = synth.gen_picture(rng, W, H, bd, ctu=ctu, dst_slot=4, intra_frac=1.0)
+        want, _ = oracle_decompress(oracle, g, dpb, pic)
+
+        def decode_and_check():
+            with intra_kernel(kernel): h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"]))
+            assert h >= 0, b200.b200_last_error()
+            vvdec_b200.check(b200.b200_wait_picture(ctx, h, None, 0))
+            got = [np.zeros_like(p) for p in want]
+            vvdec_b200.check(b200.b200_get_frame(ctx, 4, abi.plane_ptrs(got)))
+            for c in range(3): assert np.array_equal(want[c], got[c]), f"plane {c}: {len(np.argwhere(want[c] != got[c]))} diffs"
+
+        recs = pic["intraTus"]
+        for comp, x, y, l2w, l2h in ((0, 56, 0, 4, 3), (0, 64, 60, 2, 3), (1, 24, 8, 4, 2), (2, 40, 28, 2, 3)):
+            i = int(np.flatnonzero(recs["comp"] == comp)[0]); keep = recs[i].copy()
+            recs[i]["x"], recs[i]["y"], recs[i]["log2w"], recs[i]["log2h"], recs[i]["numAbove"], recs[i]["numLeft"], recs[i]["flags"] = x, y, l2w, l2h, 0, 0, 0
+            recs[i]["mode"], recs[i]["multiRefIdx"], recs[i]["mip"], recs[i]["ciip"] = 0, 0, 0, 0
+            with intra_kernel(kernel):
+                assert b200.b200_decompress_picture(ctx, C.byref(pic["struct"])) == -2 and b"intra block record" in b200.b200_last_error(), (comp, x, y)
+            recs[i] = keep
+        decode_and_check()
+
+        # one valid luma block repeated 3100 times, in the first CTU
+        i = int(np.flatnonzero((recs["comp"] == 0) & (recs["x"] == 0) & (recs["y"] == 0))[0])
+        many = np.ascontiguousarray(np.repeat(recs[i:i + 1], 3100))
+        st = pic["struct"]; keep_ptr, keep_n = st.intraTus, st.numIntraTus
+        st.intraTus, st.numIntraTus = many.ctypes.data, len(many)
+        with intra_kernel(kernel): h = b200.b200_decompress_picture(ctx, C.byref(st))
+        assert h >= 0, b200.b200_last_error()
+        rc = b200.b200_wait_picture(ctx, h, None, 0)
+        if kernel == "v1": assert rc == 0, b200.b200_last_error()
+        else: assert rc == -2 and b"more than 3072" in b200.b200_last_error()
+        st.intraTus, st.numIntraTus = keep_ptr, keep_n
+        decode_and_check()
+    finally:
+        b200.b200_ctx_destroy(ctx)
+
+
+def test_strided_copies_of_planes_that_start_in_a_registered_page(b200):
+    """b200_ctx_load_slot_strided / b200_get_frame_strided with host planes whose first page the caller has registered for another array (cudaHostRegister
+    pins whole pages; the glue pins its work-list vectors, which share the heap with the picture buffers): the planes run past that registration, and the
+    copies still move every sample."""
+    rng = np.random.default_rng(12)
+    W, H, bd, margin = 416, 240, 10, 16
+    g = abi.make_geom(W, H, bd)
+    page = 4096
+    want = synth.noise_planes(rng, W, H, bd)
+    bufs, planes, outs = [], [], []
+    for c, p in enumerate(want):
+        h, w = p.shape
+        raw = np.zeros(2 * page + (h * (w + margin) + page) * 2, np.uint8)
+        base = (-raw.ctypes.data) % page                          # a page-aligned page, then the plane starting inside the next one
+        assert b200.b200_host_register(raw.ctypes.data + base, page) == 0
+        bufs.append((raw, raw.ctypes.data + base))
+        off = base + page - 64 if c == 0 else base + 256                  # luma: the registered page's last 64 bytes; chroma: near its start
+        view = raw[off:off + h * (w + margin) * 2].view(np.int16).reshape(h, w + margin)
+        view[:, :w] = p; planes.append(view)
+    ctx = C.c_void_p()
+    try:
+        vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 2, 2, -1))
+        strides = (C.c_ssize_t * 3)(*(v.shape[1] for v in planes))
+        vvdec_b200.check(b200.b200_ctx_load_slot_strided(ctx, 0, abi.plane_ptrs(planes), strides))
+        got = [np.zeros_like(p) for p in want]
+        vvdec_b200.check(b200.b200_get_frame(ctx, 0, abi.plane_ptrs(got)))
+        for c in range(3): assert np.array_equal(got[c], want[c]), f"load plane {c}"
+        for v in planes: v[...] = 0
+        vvdec_b200.check(b200.b200_get_frame_strided(ctx, 0, abi.plane_ptrs(planes), strides))
+        for c in range(3): assert np.array_equal(planes[c][:, :want[c].shape[1]], want[c]), f"get plane {c}"
+    finally:
+        if ctx: b200.b200_ctx_destroy(ctx)
+        for raw, ptr in bufs: b200.b200_host_unregister(ptr)

@@ -194,9 +194,15 @@ B200_API int b200_intra_reconstruct(const b200_geom* g, int16_t* const planes[3]
   for (size_t i = 0; i < numTus; i++) {                      // kernel-level wrapper: records are checked here (the picture path checks on the device)
     const b200_intra_tu& t = tus[i];
     const int w = 1 << t.log2w, h = 1 << t.log2h, pw = t.comp ? g->width >> 1 : g->width, ph = t.comp ? g->height >> 1 : g->height, unit = t.comp ? 2 : 4;
-    if (t.flags & B200_INTRA_ISP) { B200_CHECK(intra_isp_record_ok(t, i ? &tus[i - 1] : nullptr, g->width, g->height), "b200_intra_reconstruct: record %zu: bad ISP region", i); continue; }
+    const bool inCtu = intra_record_in_ctu(t, intra_ctu_log2(*g));
+    if (t.flags & B200_INTRA_ISP) {
+      B200_CHECK(intra_isp_record_ok(t, i ? &tus[i - 1] : nullptr, g->width, g->height), "b200_intra_reconstruct: record %zu: bad ISP region", i);
+      B200_CHECK(inCtu, "b200_intra_reconstruct: intra block record %zu is not inside one CTU", i);
+      continue;
+    }
     B200_CHECK(t.comp < nPl && t.log2w >= 2 && t.log2w <= 6 && t.log2h >= 1 && t.log2h <= 6 && t.x + w <= pw && t.y + h <= ph && !(t.x % unit) && !(t.y % unit),
                "b200_intra_reconstruct: record %zu: bad geometry", i);
+    B200_CHECK(inCtu, "b200_intra_reconstruct: intra block record %zu is not inside one CTU", i);
     B200_CHECK(t.mode <= B200_INTRA_MDLM_T && t.multiRefIdx <= 2 && (!t.multiRefIdx || !t.comp), "b200_intra_reconstruct: record %zu: bad mode / reference line", i);
     B200_CHECK(!t.ciip || (t.ciip <= 3 && t.mode == B200_INTRA_PLANAR), "b200_intra_reconstruct: record %zu: bad CIIP block", i);
     B200_CHECK(t.mode < B200_INTRA_LM || (t.comp && t.log2w <= 5 && t.log2h <= 5 && t.lmAbove <= w && t.lmLeft <= h && (!(t.flags & B200_INTRA_LM_ABOVE) || t.y >= 2) && (!(t.flags & B200_INTRA_LM_LEFT) || t.x >= 2)
@@ -236,6 +242,7 @@ B200_API int b200_intra_reconstruct(const b200_geom* g, int16_t* const planes[3]
   if (numTus) B200_CUDA(cudaMemcpyAsync(&err, L.sync + numTus + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
   if (int rc = download_planes(g, planes, L.planes, s)) return rc;
   B200_CUDA(cudaStreamSynchronize(s));
+  B200_CHECK(!(err & INTRA_ERR_CTU_BLOCKS), "b200_intra_reconstruct: a CTU holds more than %d intra block records (overlapping records?)", INTRA_MAX_CTU_BLOCKS);
   B200_CHECK(!err, "b200_intra_reconstruct: a block waited for a neighbour that never finished, or the blocks of a CTU are not contiguous (list not in decoding order?)");
   return 0;
 }

@@ -175,6 +175,14 @@ struct IntraLaunch { b200_geom geom; DevPlanes planes; const int16_t* resi[3]; c
                                                 // the chroma residual scale of a VPDU is derived from the finished luma, so luma goes first)
                    };
 inline size_t intra_order_ints(const b200_geom& g, size_t numTus) { return numTus + 8 + 3 * (size_t)((g.width + g.ctuSize - 1) / g.ctuSize) * ((g.height + g.ctuSize - 1) / g.ctuSize); }
+inline int intra_ctu_log2(const b200_geom& g) { return g.ctuSize == 128 ? 7 : g.ctuSize == 64 ? 6 : 5; }
+// the block (or ISP region) of a record lies inside one CTU (chroma: CTU size halved): the CTU-resident kernel addresses its tile by the CTU of the
+// block's top-left sample, so a block reaching into the next CTU would write outside its tile rows
+__host__ __device__ inline bool intra_record_in_ctu(const b200_intra_tu& t, int ctuLog2)
+{
+  const int cl = ctuLog2 - (t.comp ? 1 : 0);
+  return (t.x >> cl) == ((t.x + (1 << t.log2w) - 1) >> cl) && (t.y >> cl) == ((t.y + (1 << t.log2h) - 1) >> cl);
+}
 // ISP region record (B200_INTRA_ISP, include/vvdec_b200.h): everything K6 derives addresses from.  prev = the record before it in the list (null for the first).
 __host__ __device__ inline bool intra_isp_record_ok(const b200_intra_tu& t, const b200_intra_tu* prev, int W, int H)
 {
@@ -193,6 +201,9 @@ __host__ __device__ inline bool intra_isp_record_ok(const b200_intra_tu& t, cons
 int launch_intra(const IntraLaunch& L, cudaStream_t s);
 int launch_intra_ciip_clear(const b200_intra_tu* tus, size_t numTus, int16_t* const resi[3], const int stride[3], cudaStream_t s);   // before K1: see k6_intra.cu
 int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_geom& g, int* meta, cudaStream_t s);   // error bit 8 of the PU meta block (after launch_mc_bucket)
+// K6 error word (sync[numTus + 1]): bit 1 a wait timed out, bit 2 the blocks of a CTU are not contiguous in the list, bit 4 a CTU holds more blocks than the
+// CTU-resident kernel has done bytes for (V2_FLAGS = 3072; only that kernel checks it, and it runs nothing when bit 2 or 4 is set)
+constexpr int INTRA_ERR_ORDER = 2, INTRA_ERR_CTU_BLOCKS = 4, INTRA_MAX_CTU_BLOCKS = 3072;
 int launch_film_grain(const DevPlanes& src, const DevPlanes& dst, const b200_geom& g, const int8_t* pattern, const uint8_t* sLUT, const uint8_t* pLUT,
                       const uint32_t* lineSeeds, uint32_t* seeds, int scaleShift, const uint8_t present[3], cudaStream_t s);   // film_grain.cu
 int launch_hash(const DevPlanes& src, const b200_geom& g, int method, uint32_t* acc, uint8_t* digest, cudaStream_t s);   // hash.cu: CRC / checksum of the planes

@@ -460,7 +460,8 @@ __global__ void __launch_bounds__(IT_THREADS, 12) intra_kernel(const IntraParams
 constexpr int V2_LS = 136, V2_CS = 72;                       // tile row pitch in samples: a multiple of 16 bytes (16-byte asynchronous copies), rows 4 banks apart
 constexpr int V2_TILE = 128 * V2_LS + 2 * 64 * V2_CS;        // samples of one tile set (Y, Cb, Cr)
 constexpr int V2_RECS = 1024;                                // records staged in shared memory (a CTU with more blocks reads the rest from global memory)
-constexpr int V2_FLAGS = 128 * 128 / 16 + 2 * (64 * 64 / 4); // most blocks a CTU can hold
+constexpr int V2_FLAGS = 128 * 128 / 16 + 2 * (64 * 64 / 4); // most blocks a CTU can hold without overlapping records (a list with more is refused)
+static_assert(V2_FLAGS == INTRA_MAX_CTU_BLOCKS, "the documented per-CTU block limit is the number of done bytes");
 struct V2Scratch { int16_t T[2][IT_REF], L[2][IT_REF], M[IT_ARR], S[IT_ARR], Lm[32 * 32], LmTop[64], LmLeft[64]; int LmPar[4]; int next[2], sum; };
 constexpr int V2_OWN = 3 * 32 * 32;                         // owner words of the CTU's units: luma 32 x 32 (4x4 units), Cb / Cr 32 x 32 each (2x2 units)
 constexpr size_t v2_smem(int groups) { return (size_t)2 * V2_TILE * sizeof(int16_t) + groups * sizeof(V2Scratch) + V2_RECS * sizeof(b200_intra_tu) + V2_OWN * sizeof(int) + V2_FLAGS + 64; }
@@ -494,13 +495,15 @@ __global__ void __launch_bounds__(1024) intra_ctu_order_kernel(const IntraParams
   }
   if (threadIdx.x == 0) { int m = 0; for (int j = 0; j < n; j++) m += sCnt[j] > 0; counters[0] = m; counters[1] = 0; }
 }
-// contiguity of every CTU's blocks in the list (decoding order): entry i belongs to the run [ctuFirst, ctuFirst + ctuCnt) of its CTU
+// contiguity of every CTU's blocks in the list (decoding order): entry i belongs to the run [ctuFirst, ctuFirst + ctuCnt) of its CTU; and no CTU holds more
+// blocks than intra_ctu_kernel has done bytes for (only overlapping records get there)
 __global__ void __launch_bounds__(256) intra_ctu_check_kernel(const IntraParams P)
 {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= P.numTus) return;
   const int c = intra_ctu_of(P, P.tus[i]);
-  if (i - P.ctuFirst[c] >= P.ctuCnt[c]) atomicOr(P.err, 2);
+  if (i - P.ctuFirst[c] >= P.ctuCnt[c]) atomicOr(P.err, INTRA_ERR_ORDER);
+  if (i == P.ctuFirst[c] && P.ctuCnt[c] > V2_FLAGS) atomicOr(P.err, INTRA_ERR_CTU_BLOCKS);
 }
 
 __device__ __forceinline__ int v2_ld_acquire(const int* p) { int v; asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
@@ -548,7 +551,8 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
     __syncthreads();
     if (tid == 0) { sCtu = atomicAdd(&counters[1], 1); sNext = V2_GROUPS; }
     __syncthreads();
-    if (sCtu >= counters[0] || (*(volatile int*)P.err & 2)) return;          // bit 2: a CTU's blocks are not contiguous in the list (intra_ctu_check_kernel)
+    if (sCtu >= counters[0] || (*(volatile int*)P.err & (INTRA_ERR_ORDER | INTRA_ERR_CTU_BLOCKS))) return;   // intra_ctu_check_kernel: a CTU's blocks are not
+                                                                             // contiguous in the list, or more than sflag holds: nothing is staged
     const int ctu = ctuOrder[sCtu], first = P.ctuFirst[ctu], cnt = P.ctuCnt[ctu];
     long long tp = clock64(); (void)tp;
     // the CTU's luma origin and extent; component c's tile is these >> (c ? 1 : 0), at v2_tile_off(c) in the tile sets (plain values, not arrays indexed by
@@ -911,11 +915,12 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
 }
 
 // record checks of the picture path (the kernel-level wrapper checks on the host): everything K6 uses as an address
-__global__ void __launch_bounds__(256) intra_validate_kernel(const b200_intra_tu* __restrict__ tus, int n, int W, int H, int chroma, int* meta)
+__global__ void __launch_bounds__(256) intra_validate_kernel(const b200_intra_tu* __restrict__ tus, int n, int W, int H, int chroma, int ctuLog2, int* meta)
 {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= n) return;
   const b200_intra_tu t = tus[i];
+  if (!intra_record_in_ctu(t, ctuLog2)) { atomicOr(&meta[LM_ERR], 8); return; }
   if (t.flags & B200_INTRA_ISP) { b200_intra_tu prev; if (i) prev = tus[i - 1]; if (!intra_isp_record_ok(t, i ? &prev : nullptr, W, H)) atomicOr(&meta[LM_ERR], 8); return; }
   const int w = 1 << t.log2w, h = 1 << t.log2h, pw = t.comp ? W >> 1 : W, ph = t.comp ? H >> 1 : H, unit = t.comp ? 2 : 4, m = t.multiRefIdx;
   bool ok = t.comp < (chroma ? 3 : 1) && t.log2w >= 2 && t.log2w <= 6 && t.log2h >= 1 && t.log2h <= 6 && t.x + w <= pw && t.y + h <= ph && !(t.x % unit) && !(t.y % unit);
@@ -969,7 +974,7 @@ int launch_intra_ciip_clear(const b200_intra_tu* tus, size_t numTus, int16_t* co
 int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_geom& g, int* meta, cudaStream_t s)
 {
   if (!numTus) return 0;
-  intra_validate_kernel<<<(unsigned)((numTus + 255) / 256), 256, 0, s>>>(tus, (int)numTus, g.width, g.height, g.chromaFormat != 0, meta);
+  intra_validate_kernel<<<(unsigned)((numTus + 255) / 256), 256, 0, s>>>(tus, (int)numTus, g.width, g.height, g.chromaFormat != 0, intra_ctu_log2(g), meta);
   B200_CUDA(cudaGetLastError());
   return 0;
 }
@@ -993,12 +998,15 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
     for (int c = 0; c < (L.geom.chromaFormat ? 3 : 1); c++) B200_CUDA(cudaMemsetAsync(L.owner[c], 0xff, L.ownerBytes[c], s));
   }
   P.perm = nullptr; P.ctuCnt = P.ctuFirst = P.ctuBase = nullptr;
-  P.ctuLog2 = L.geom.ctuSize == 128 ? 7 : L.geom.ctuSize == 64 ? 6 : 5; P.ctusW = (L.geom.width + L.geom.ctuSize - 1) / L.geom.ctuSize; P.ctusH = (L.geom.height + L.geom.ctuSize - 1) / L.geom.ctuSize;
-  static const char* variant = getenv("B200_INTRA_KERNEL");      // measurement switch: "v1" = one CTA per block through global memory (round 1)
-  // v2 (CTU-resident) shortens the dependency chains of dense lists (I pictures); the scattered intra CUs of a B picture have almost no chains and
-  // finish sooner with v1's one-CTA-per-block throughput (measured at 4K: 15 % intra CUs 0.08 ms vs 0.24 ms; I picture 12.5 ms vs 8 ms)
+  P.ctuLog2 = intra_ctu_log2(L.geom); P.ctusW = (L.geom.width + L.geom.ctuSize - 1) / L.geom.ctuSize; P.ctusH = (L.geom.height + L.geom.ctuSize - 1) / L.geom.ctuSize;
+  // Measurement and test switch, read on every launch (one getenv per picture): B200_INTRA_KERNEL=v1 (one CTA per block through global memory) or v2
+  // (CTU-resident); unset or any other value: chosen by density.  v2 (CTU-resident) shortens the dependency chains of dense lists (I pictures); the
+  // scattered intra CUs of a B picture have almost no chains and finish sooner with v1's one-CTA-per-block throughput (measured at 4K: 15 % intra CUs
+  // 0.08 ms vs 0.24 ms; I picture 12.5 ms vs 8 ms).  Both launches of an LMCS two-pass picture take the same kernel: compSel 2 reuses the first one's order scratch.
+  const char* variant = getenv("B200_INTRA_KERNEL");
+  const bool force1 = variant && !strcmp(variant, "v1"), force2 = variant && !strcmp(variant, "v2");
   const bool dense = L.numTus >= 48 * std::max<size_t>(1, (size_t)L.geom.width * L.geom.height >> 14);                   // >= 48 blocks per 128x128 luma area
-  const bool v1 = !L.order || (variant ? !strcmp(variant, "v1") : !dense) || ((P.stride[0] | P.stride[1] | P.stride[2]) & 1);   // the tile loads move 32-bit words
+  const bool v1 = !L.order || force1 || (!force2 && !dense) || ((P.stride[0] | P.stride[1] | P.stride[2]) & 1);          // the tile loads move 32-bit words
   const unsigned grid = (unsigned)((L.numTus + 255) / 256);
   if (!cont) intra_owner_kernel<<<(unsigned)L.numTus, 64, 0, s>>>(P);
   if (!v1) {
@@ -1034,7 +1042,8 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
     B200_CUDA(cudaGetLastError());
     return 0;
   }
-  static const bool listOrder = getenv("B200_INTRA_ORDER") && !strcmp(getenv("B200_INTRA_ORDER"), "decode");   // measurement switch: tickets in list order
+  const char* order = getenv("B200_INTRA_ORDER");                // measurement and test switch, read on every launch: "decode" = tickets in list order
+  const bool listOrder = order && !strcmp(order, "decode");
   if (L.order && !listOrder && L.numTus >= 100 * std::max<size_t>(1, (size_t)L.geom.width * L.geom.height >> 14)) {   // >= 100 blocks per 128x128 luma area
     const size_t nCtu = (size_t)P.ctusW * P.ctusH;
     int* perm = L.order; P.ctuCnt = perm + L.numTus; P.ctuFirst = P.ctuCnt + nCtu; P.ctuBase = P.ctuFirst + nCtu;

@@ -393,8 +393,11 @@ B200_API int b200_wait_picture(b200_ctx* c, int ai, int32_t* dmvrMv, size_t numD
   }
   B200_CUDA(cudaStreamSynchronize(c->upStream));
   B200_CUDA(cudaStreamSynchronize(c->stream));
-  if (ai >= 0 && ai < c->numArenas && c->arenas[ai].numIntraTus)
-    B200_CHECK(!c->arenas[ai].hMeta[2 * LM_INTS], "b200_wait_picture: an intra block waited for a neighbour that never finished (intra list not in decoding order?)");
+  if (ai >= 0 && ai < c->numArenas && c->arenas[ai].numIntraTus) {
+    const int err = c->arenas[ai].hMeta[2 * LM_INTS];
+    B200_CHECK(!(err & INTRA_ERR_CTU_BLOCKS), "b200_wait_picture: a CTU holds more than %d intra block records (overlapping records?)", INTRA_MAX_CTU_BLOCKS);
+    B200_CHECK(!err, "b200_wait_picture: an intra block waited for a neighbour that never finished (intra list not in decoding order?)");
+  }
   return 0;
 }
 
@@ -409,6 +412,32 @@ B200_API int b200_get_frame(b200_ctx* c, int slot, int16_t* const planes[3])
 }
 
 // Picture buffers of the host decoder carry margins (stride > width): 2-D copies between the margin-less device planes and strided host planes.
+// The runtime classifies a host range by its first address.  cudaHostRegister pins whole pages, so a plane that starts on a page the caller registered for
+// another array (the glue pins its work-list vectors, which share the heap with the decoder's picture buffers) and runs past that registration is refused with
+// cudaErrorInvalidValue.  Such a plane goes through a pinned staging copy instead.
+static int copy2d_host(void* dst, size_t dpitch, const void* src, size_t spitch, size_t wBytes, size_t h, cudaMemcpyKind kind, cudaStream_t s)
+{
+  const cudaError_t e = cudaMemcpy2DAsync(dst, dpitch, src, spitch, wBytes, h, kind, s);
+  if (e != cudaErrorInvalidValue) { B200_CUDA(e); return 0; }
+  (void)cudaGetLastError();
+  void* stage = nullptr;
+  B200_CUDA(cudaMallocHost(&stage, wBytes * h));
+  int rc = 0;
+  if (kind == cudaMemcpyHostToDevice) {
+    for (size_t y = 0; y < h; y++) memcpy((char*)stage + y * wBytes, (const char*)src + y * spitch, wBytes);
+    const cudaError_t e2 = cudaMemcpy2DAsync(dst, dpitch, stage, wBytes, wBytes, h, kind, s);
+    const cudaError_t e3 = e2 == cudaSuccess ? cudaStreamSynchronize(s) : e2;
+    if (e3 != cudaSuccess) { set_error("copy2d_host: staged H2D copy -> %s", cudaGetErrorString(e3)); (void)cudaGetLastError(); rc = B200_ERR_CUDA; }
+  } else {
+    const cudaError_t e2 = cudaMemcpy2DAsync(stage, wBytes, src, spitch, wBytes, h, kind, s);
+    const cudaError_t e3 = e2 == cudaSuccess ? cudaStreamSynchronize(s) : e2;
+    if (e3 != cudaSuccess) { set_error("copy2d_host: staged D2H copy -> %s", cudaGetErrorString(e3)); (void)cudaGetLastError(); rc = B200_ERR_CUDA; }
+    else for (size_t y = 0; y < h; y++) memcpy((char*)dst + y * dpitch, (const char*)stage + y * wBytes, wBytes);
+  }
+  cudaFreeHost(stage);
+  return rc;
+}
+
 B200_API int b200_ctx_load_slot_strided(b200_ctx* c, int slot, const int16_t* const planes[3], const ptrdiff_t strides[3])
 {
   B200_CHECK(c && planes && strides && slot >= 0 && slot < c->numSlots, "b200_ctx_load_slot_strided: bad argument");
@@ -416,7 +445,7 @@ B200_API int b200_ctx_load_slot_strided(b200_ctx* c, int slot, const int16_t* co
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++) {
     const size_t w = k ? c->g.width >> 1 : c->g.width, h = k ? c->g.height >> 1 : c->g.height;
     B200_CHECK(planes[k] && strides[k] >= (ptrdiff_t)w, "b200_ctx_load_slot_strided: plane %d", k);
-    B200_CUDA(cudaMemcpy2DAsync(d.p[k], (size_t)c->g.stride[k] * 2, planes[k], (size_t)strides[k] * 2, w * 2, h, cudaMemcpyHostToDevice, c->stream));
+    if (int rc = copy2d_host(d.p[k], (size_t)c->g.stride[k] * 2, planes[k], (size_t)strides[k] * 2, w * 2, h, cudaMemcpyHostToDevice, c->stream)) return rc;
   }
   B200_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
@@ -429,7 +458,7 @@ B200_API int b200_get_frame_strided(b200_ctx* c, int slot, int16_t* const planes
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++) {
     const size_t w = k ? c->g.width >> 1 : c->g.width, h = k ? c->g.height >> 1 : c->g.height;
     B200_CHECK(planes[k] && strides[k] >= (ptrdiff_t)w, "b200_get_frame_strided: plane %d", k);
-    B200_CUDA(cudaMemcpy2DAsync(planes[k], (size_t)strides[k] * 2, d.p[k], (size_t)c->g.stride[k] * 2, w * 2, h, cudaMemcpyDeviceToHost, c->stream));
+    if (int rc = copy2d_host(planes[k], (size_t)strides[k] * 2, d.p[k], (size_t)c->g.stride[k] * 2, w * 2, h, cudaMemcpyDeviceToHost, c->stream)) return rc;
   }
   B200_CUDA(cudaStreamSynchronize(c->stream));
   return 0;

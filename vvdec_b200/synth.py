@@ -508,7 +508,7 @@ def gen_picture(rng, W, H, bit_depth=10, ctu=128, dst_slot=0, cu_kw=None, pu_kw=
         tus, coefs = np.concatenate([tus0, tus1, tus2]), np.concatenate([coefs0, coefs1, coefs2])
         mask = is_intra.copy()
         for i in ciip: mask[i] = True
-        irecs = gen_intra_records(rng, cus, W, H, only=mask, p_lm=0.2, colloc=int(rng.integers(0, 2)), ciip=ciip)
+        irecs = gen_intra_records(rng, cus, W, H, only=mask, p_lm=0.2, colloc=int(rng.integers(0, 2)), ciip=ciip, ctu=ctu)
         coded = set()
         for t in np.concatenate([tus1, tus2[(tus2["flags"] & A.TU_RESI) != 0]]):
             coded.add((int(t["comp"]), int(t["x"]), int(t["y"]))); 
@@ -697,11 +697,11 @@ def isp_regions(w, h, split):
     return [(k * rw, 0, rw, h) for k in range(w // rw)], part
 
 
-def gen_intra_records(rng, layout, W, H, modes=None, p_mrl=0.15, p_bdpcm=0.08, p_resi=0.0, upto=None, only=None, p_mip=0.15, colloc=0, p_lm=0.0, ciip=None, p_isp=0.0):
+def gen_intra_records(rng, layout, W, H, modes=None, p_mrl=0.15, p_bdpcm=0.08, p_resi=0.0, upto=None, only=None, p_mip=0.15, colloc=0, p_lm=0.0, ciip=None, p_isp=0.0, ctu=128):
     """b200_intra_tu records (Y, Cb, Cr per CU, decoding order) for a single-tree all-intra layout of gen_intra_layout: random modes, MRL on some luma
-    blocks, BDPCM prediction on some, availability as xFillReferenceSamples derives it from the decoding order (pinned against the reference's own
-    analysis through the glue flattener by tests/test_intra_oracle_vs_ref.py).  Luma blocks whose chroma would be narrower than 4 or smaller than 16
-    samples are luma-only (local dual tree; their chroma is not generated)."""
+    blocks (never on the first row of a CTU of size `ctu`, the layout's), BDPCM prediction on some, availability as xFillReferenceSamples derives it
+    from the decoding order (pinned against the reference's own analysis through the glue flattener by tests/test_intra_oracle_vs_ref.py).  Luma blocks
+    whose chroma would be narrower than 4 or smaller than 16 samples are luma-only (local dual tree; their chroma is not generated)."""
     A = abi
     owner = np.full(((H + 3) // 4, (W + 3) // 4), 1 << 30, np.int64)
     for i, (x, y, w, h) in enumerate(layout): owner[y // 4:(y + h) // 4, x // 4:(x + w) // 4] = i
@@ -713,7 +713,7 @@ def gen_intra_records(rng, layout, W, H, modes=None, p_mrl=0.15, p_bdpcm=0.08, p
             m = modes[i]; dirL, dirC, mrl, bdpcm = m[:4]; mip = m[4] if len(m) > 4 else 0
         else:
             dirL, mrl, bdpcm = int(rng.integers(0, 67)), 0, 0
-            if rng.random() < p_mrl and y % 128: mrl, dirL = int(rng.integers(1, 3)), int(rng.integers(1, 67))
+            if rng.random() < p_mrl and y % ctu: mrl, dirL = int(rng.integers(1, 3)), int(rng.integers(1, 67))
             elif rng.random() < p_bdpcm and w <= 32 and h <= 32: bdpcm = int(rng.integers(1, 3))
             elif rng.random() < p_mip:                                   # matrix intra prediction: dirL is the MIP mode index of the size class
                 n_modes = 16 if (w, h) == (4, 4) else 8 if (w == 4 or h == 4 or (w, h) == (8, 8)) else 6
@@ -771,3 +771,89 @@ def gen_intra_records(rng, layout, W, H, modes=None, p_mrl=0.15, p_bdpcm=0.08, p
             r["flags"], r["numAbove"], r["numLeft"] = fl, na, nl
             recs.append(r)
     return np.array(recs, A.INTRA_TU_DTYPE)
+
+
+# ---------------------------------------------------------------------------------------------------------------- designed intra sweep
+def intra_sweep_blocks():
+    """The blocks of the designed K6 sweep, as (comp, w, h, mode, multiRefIdx, mip): every luma shape 4x4 .. 64x64 with every mode 0..66, MRL 1 and 2 with
+    every angular mode, BDPCM H / V up to 32x32 and every MIP mode of the size class, transposed and not; every chroma shape 4x4 .. 32x32 of Cb and Cr with
+    every mode 0..66."""
+    A = abi
+    out = []
+    sizes = (4, 8, 16, 32, 64)
+    for w in sizes:
+        for h in sizes:
+            out += [(0, w, h, m, 0, 0) for m in range(67)]
+            out += [(0, w, h, m, mrl, 0) for mrl in (1, 2) for m in range(2, 67)]
+            if w <= 32 and h <= 32: out += [(0, w, h, A.INTRA_BDPCM_HOR, 0, 0), (0, w, h, A.INTRA_BDPCM_VER, 0, 0)]
+            n_mip = 16 if (w, h) == (4, 4) else 8 if (w == 4 or h == 4 or (w, h) == (8, 8)) else 6
+            out += [(0, w, h, A.INTRA_MIP, 0, k | (tr << 7)) for k in range(n_mip) for tr in (0, 1)]
+    for c in (1, 2):
+        out += [(c, w, h, m, 0, 0) for w in sizes[:4] for h in sizes[:4] for m in range(67)]
+    return out
+
+
+INTRA_SWEEP_AVAIL = ("full", "partial", "none")
+
+
+def _sweep_slots(cx, cy, C, W, H, w, h, gap):
+    """Positions of a w x h block grid inside the CTU (cx, cy, size C) of a W x H plane.  Every block keeps `gap` free columns left of it and `gap` free rows
+    above it (its reference row / column, MRL lines included), and its above-right and below-left references (2w, 2h) end inside the CTU or the free band
+    in front of the next CTU.  So no block's reference samples are another block's samples: every reference is noise, nothing depends on anything."""
+    xs = [x for x in range(cx + gap, cx + C, w + gap) if x + w <= cx + C and x + 2 * w <= min(cx + C + gap, W)]
+    ys = [y for y in range(cy + gap, cy + C, h + gap) if y + h <= cy + C and y + 2 * h <= min(cy + C + gap, H)]
+    return [(x, y) for y in ys for x in xs]
+
+
+def intra_sweep(ctu=128, ctus_w=32):
+    """The designed sweep as one list: every block of intra_sweep_blocks() once per neighbourhood of INTRA_SWEEP_AVAIL (full: numAbove = 2w / unit,
+    numLeft = 2h / unit and the corner; partial: above-right or below-left cut, no corner; none), placed on a grid of noise in CTU raster order with each
+    CTU's records contiguous (luma, Cb, Cr).  Luma reference filtering as intra_filter_ref says; every record carries INTRA_ADD_RESI.
+    Returns (W, H, records); the picture is ctus_w CTUs wide and has one empty CTU row at the bottom."""
+    A = abi
+    blocks = intra_sweep_blocks()
+    groups = {}                                                   # (luma?, w, h) -> [(comp, mode, mrl, mip, avail)], Cb and Cr of a shape side by side
+    for (c, w, h, mode, mrl, mip) in blocks:
+        for av in INTRA_SWEEP_AVAIL: groups.setdefault((c == 0, w, h), []).append((c, mode, mrl, mip, av))
+    W = ctus_w * ctu
+    per_ctu = {}                                                  # CTU index -> records
+    for luma in (True, False):
+        C, gap, sh = (ctu, 4, 0) if luma else (ctu // 2, 2, 1)
+        Wc = W >> sh
+        k = 0                                                     # next CTU of this channel
+        for (l, w, h), todo in groups.items():
+            if l != luma: continue
+            cr = None if luma else [b for b in todo if b[0] == 2]  # Cr blocks at the positions of the Cb blocks, in their own plane
+            if not luma: todo = [b for b in todo if b[0] == 1]
+            i = 0
+            while i < len(todo):
+                cx, cy = (k % ctus_w) * C, (k // ctus_w) * C
+                slots = _sweep_slots(cx, cy, C, Wc, 1 << 30, w, h, gap)
+                for (x, y) in slots:
+                    if i >= len(todo): break
+                    for b in ([todo[i]] if luma else [todo[i], cr[i]]):
+                        per_ctu.setdefault(k, []).append((b[0], x, y, w, h) + b[1:])
+                    i += 1
+                k += 1
+    n_ctu = max(per_ctu) + 1
+    H = ((n_ctu + ctus_w - 1) // ctus_w + 1) * ctu
+    recs = []
+    for k in sorted(per_ctu):
+        for j, (c, x, y, w, h, mode, mrl, mip, av) in enumerate(sorted(per_ctu[k], key=lambda r: r[0])):
+            r = np.zeros((), A.INTRA_TU_DTYPE)
+            unit = 2 if c else 4
+            r["x"], r["y"], r["log2w"], r["log2h"], r["comp"], r["mode"], r["multiRefIdx"], r["mip"] = x, y, int(np.log2(w)), int(np.log2(h)), c, mode, mrl, mip
+            fl = A.INTRA_ADD_RESI
+            if av == "full": fl |= A.INTRA_AVAIL_TL; r["numAbove"], r["numLeft"] = 2 * w // unit, 2 * h // unit
+            elif av == "partial":
+                if j & 1: r["numAbove"], r["numLeft"] = w // unit, 2 * h // unit
+                else: r["numAbove"], r["numLeft"] = 2 * w // unit, h // unit
+            if c == 0 and mode <= 66 and intra_filter_ref(w, h, mode, mrl, 0): fl |= A.INTRA_FILTER_REF
+            r["flags"] = fl
+            recs.append(r)
+    return W, H, np.array(recs, A.INTRA_TU_DTYPE)
+
+
+def intra_record_key(r):
+    """(comp, w, h, mode, multiRefIdx, mip) of a record: the block identity intra_sweep_blocks() lists."""
+    return (int(r["comp"]), 1 << int(r["log2w"]), 1 << int(r["log2h"]), int(r["mode"]), int(r["multiRefIdx"]), int(r["mip"]))
