@@ -253,7 +253,12 @@ typedef struct b200_wp {
  * picture (only PU areas are written).  dmvrMv: int32 [n][2] (hor,ver deltas, Mv layout of m_dmvrMvCache), may be NULL. */
 B200_API int b200_mc_predict(const b200_geom* g, int16_t* const dst[3], const int16_t* const* refs, int numSlots,
                              const b200_pu* pus, size_t numPus, int32_t* dmvrMv, size_t numDmvr);
-/* the same with an explicit-weighted-prediction table (wp may be NULL when no PU has wpIdx != 0) */
+/* the same with an explicit-weighted-prediction table (wp may be NULL when no PU has wpIdx != 0).
+ * Both return B200_ERR_PARAM, with dst and dmvrMv untouched, for a chromaFormat other than 0 (4:0:0) or 1 (4:2:0), a bit depth outside 8..12, a plane
+ * stride smaller than its plane's width, and for any PU the list validation refuses: reference slots outside [0, numSlots) or none, a side that is not a
+ * multiple of 4 in 4..128 or leaves a 12-sample tile (12, 28, 44, ...), a block off the 4x4 grid or outside the picture, DMVR entries past numDmvr, DMVR on a uni-predicted, affine or
+ * smaller than 8x8 / 128-sample PU, BDOF on such a small bi-predicted PU, DMVR above 10 bit, GEO that is uni-predicted, outside 8..64 per side,
+ * combined with DMVR / BDOF / affine / weights or with a split direction above 63, and weights (wpIdx) past numWp or combined with DMVR, BDOF or BCW. */
 B200_API int b200_mc_predict_wp(const b200_geom* g, int16_t* const dst[3], const int16_t* const* refs, int numSlots,
                                 const b200_pu* pus, size_t numPus, int32_t* dmvrMv, size_t numDmvr, const b200_wp* wp, int numWp);
 

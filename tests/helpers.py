@@ -512,3 +512,64 @@ def intra_case(W, H, ctu, seed, min_size=8, bd=10, chroma=True, strides=None, p_
     resi = [rng.integers(-40, 41, size=p.shape).astype(np.int16) for p in planes]
     if not chroma: planes, resi = planes + [None, None], resi + [None, None]
     return g, planes, resi, recs
+
+
+# ---- K2: one comparison for every MC test (tests/test_k2_*.py)
+def mc_dst(g, fill=-1):
+    """Destination planes of a geometry (its strides, None for absent chroma), filled with a sentinel so that a sample nobody wrote stands out."""
+    out = [np.full((g.height, g.stride[0]), fill, np.int16)]
+    for c in (1, 2):
+        out.append(np.full((g.height >> 1, g.stride[c]), fill, np.int16) if g.chromaFormat else None)
+    return out
+
+
+def mc_oracle(oracle, case):
+    """orc_mc_predict_wp on a sweep case (synth.mc_sweep): (planes, DMVR deltas)."""
+    g, pus = case["g"], case["pus"]
+    a = mc_dst(g); da = np.zeros((case["ndmvr"] + 1, 2), np.int32)
+    ent = case["wp"][1] if case["wp"] else None
+    oracle.orc_mc_predict_wp(C.byref(g), abi.plane_ptrs(a), ref_ptrs(case["refs"]), pus.ctypes.data, len(pus), da.ctypes.data, None if ent is None else ent.ctypes.data)
+    return a, da
+
+
+def mc_tile_path(case, i, tx, ty):
+    """Which path tile (tx, ty) of PU i takes in k2_inter.cu: its list, and for each list of the PU whether the window of the initial MV is interior
+    (word copies) or on the boundary (per-sample clamped copies), DMVR's fast or slow search window."""
+    pu = case["pus"][i]; g = case["g"]
+    lst = synth.mc_list_of(pu, tx, ty)
+    if lst == 16: return "affine list (one thread per sample, clamped reads)"
+    tw, th = min(16, int(pu["w"]) - 16 * tx), min(16, int(pu["h"]) - 16 * ty)
+    even = all(s % 2 == 0 for s in case["strides"][:3 if case["chroma"] else 1])
+    kinds = ("dmvr", "dmvr_chroma") if lst // 4 == 3 else ("luma", "chroma")
+    parts = []
+    for l in range(2):
+        if pu["refSlot"][l] < 0: continue
+        win = synth.mc_tile_windows(pu, l, tx, ty)
+        for k in kinds[:2 if case["chroma"] else 1]:
+            x0, x1, y0, y1 = synth.mc_window_margins(k, g.width, g.height, tw, th)
+            x, y = win[k]
+            inside = even and x0 <= x <= x1 and y0 <= y <= y1
+            parts.append(f"L{l} {k} " + (("fast" if inside else "slow") + " search window" if k.startswith("dmvr") else "interior" if inside else "boundary"))
+    return f"list {lst} (mode {lst // 4}, class {lst % 4}, tile {tw}x{th}); " + ", ".join(parts)
+
+
+def mc_mismatch(case, a, b, da, db):
+    """None when the planes and DMVR deltas agree; else a message naming the case, the first differing sample, its PU and its tile's path.  The whole
+    rows are compared, stride padding included: both sides start from the same sentinel, so a store past a row's last sample shows."""
+    g = case["g"]
+    for c in range(3 if g.chromaFormat else 1):
+        A, B = a[c], b[c]
+        if not np.array_equal(A, B):
+            d = np.argwhere(A != B); y, x = (int(v) for v in d[0]); sh = 1 if c else 0
+            pus = case["pus"]
+            hit = [i for i, p in enumerate(pus) if p["x"] >> sh <= x < (p["x"] + p["w"]) >> sh and p["y"] >> sh <= y < (p["y"] + p["h"]) >> sh]
+            where = "no PU"
+            if hit:
+                i = hit[0]; p = pus[i]
+                tx, ty = ((x << sh) - int(p["x"])) // 16, ((y << sh) - int(p["y"])) // 16
+                where = f"PU {i} ({case['tags'][i]}) {p}; tile ({tx}, {ty}): {mc_tile_path(case, i, tx, ty)}"
+            return f"{case['name']}: plane {c}: {len(d)} samples differ, first at (y={y}, x={x}): {A[y, x]} vs {B[y, x]}; {where}"
+    if not np.array_equal(da, db):
+        bad = np.argwhere((da != db).any(axis=1))[:, 0]
+        return f"{case['name']}: DMVR deltas differ at entries {bad[:5].tolist()}: {da[bad[:5]].tolist()} vs {db[bad[:5]].tolist()}"
+    return None

@@ -115,3 +115,24 @@ def test_geo(oracle, ref, simd, bd):
         seen |= set(int(v) for v in geo["bcwW1"])
         _compare(oracle, ref, simd, W, H, bd, pus, ndmvr, refs)
     assert len(seen) >= 60
+
+
+@pytest.mark.parametrize("simd", [0, 1])
+@pytest.mark.parametrize("name", list(synth.MC_SWEEP_CASES))
+def test_designed_sweep(oracle, ref, name, simd):
+    """Every case of the designed K2 sweep (synth.mc_sweep: shapes x tools, phases, window thresholds at the picture edges, clipMv bounds for CTU 32 / 64
+    / 128, MVs near +-2^17, affine spread limits, DMVR targets and designed cost surfaces; 8 / 10 / 12 bit, 4:0:0, padded and odd strides): the
+    oracle and the real motion compensation give the same samples and DMVR deltas."""
+    from tests.helpers import mc_dst, mc_oracle, mc_mismatch
+    case = synth.mc_sweep(name)
+    g, pus = case["g"], case["pus"]
+    a, da = mc_oracle(oracle, case)
+    b = mc_dst(g); db = np.zeros_like(da)
+    if case["wp"]: ref.ref_set_wp(case["wp"][0].ctypes.data)
+    try:
+        rc = ref.ref_mc_predict(simd, C.byref(g), abi.plane_ptrs(b), ref_ptrs(case["refs"]), pus.ctypes.data, len(pus), db.ctypes.data, case["ndmvr"])
+    finally:
+        ref.ref_set_wp(None)
+    assert rc == 0, "the reference did not take the DMVR decision the PU flags ask for"
+    msg = mc_mismatch(case, a, b, da, db)
+    assert msg is None, msg

@@ -322,3 +322,77 @@ def test_strided_copies_of_planes_that_start_in_a_registered_page(b200):
     finally:
         if ctx: b200.b200_ctx_destroy(ctx)
         for raw, ptr in bufs: b200.b200_host_unregister(ptr)
+
+
+@pytest.mark.parametrize("name,lmcs", [("shapes_10bit", True), ("wp_10bit", True), ("edges_ctu32_stride_odd", False)])
+def test_designed_mc_lists_in_a_picture(b200, oracle, name, lmcs):
+    """Lists of the designed K2 sweep (synth.mc_sweep) through b200_decompress_picture, K2 reading the device DPB slots: with LMCS every luma store site
+    (uni, bi, BDOF, DMVR, affine uni / bi, GEO; weighted uni / bi / affine in the wp list) forward-maps; the edges list runs in a context with CTU 32 and
+    an odd luma stride.  Samples and the DMVR deltas b200_wait_picture returns match the oracle chain; the samples no PU covers come from `given`."""
+    from tests.helpers import mc_dst
+    case = synth.mc_sweep(name)
+    g, W, H, bd = case["g"], case["W"], case["H"], case["bd"]
+    ctx = C.c_void_p()
+    vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 2, -1))
+    try:
+        for s in range(4): vvdec_b200.check(b200.b200_ctx_load_slot(ctx, s, abi.plane_ptrs(case["refs"][s])))
+        pic = synth.gen_picture(np.random.default_rng(9), W, H, bd, ctu=case["ctu"], dst_slot=4, inter=False, tu_kw=dict(p_cbf=0.0), deblock=False, sao=False,
+                                alf=False, lmcs=lmcs)
+        st = pic["struct"]
+        pic["pus"], pic["ndmvr"] = case["pus"], case["ndmvr"]
+        st.pus = case["pus"].ctypes.data; st.numPus = len(case["pus"]); st.numDmvr = case["ndmvr"] + 1
+        pic["given"] = mc_dst(g, 0)
+        for c in range(3): st.given[c] = pic["given"][c].ctypes.data
+        if case["wp"]:
+            pic["wp"] = case["wp"][1]; st.wp = pic["wp"].ctypes.data; st.numWp = len(pic["wp"])
+        want, dm_want = oracle_decompress(oracle, g, case["refs"], pic)
+        h = b200.b200_decompress_picture(ctx, C.byref(st))
+        assert h >= 0, b200.b200_last_error()
+        dm = np.zeros_like(dm_want)
+        vvdec_b200.check(b200.b200_wait_picture(ctx, h, dm.ctypes.data, len(dm)))
+        got = mc_dst(g, 0)
+        vvdec_b200.check(b200.b200_get_frame(ctx, 4, abi.plane_ptrs(got)))
+        for c in range(3):
+            w, hh = (W, H) if c == 0 else (W // 2, H // 2)
+            bad = np.argwhere(want[c][:hh, :w] != got[c][:hh, :w])
+            assert len(bad) == 0, f"{name}: plane {c}: {len(bad)} diffs, first at {bad[:1].tolist()}"
+        assert np.array_equal(dm, dm_want), f"{name}: DMVR deltas differ"
+        if lmcs and name == "shapes_10bit": assert {t for t in case["tags"]} >= {"uni0", "bi", "bdof", "dmvr", "aff4_uni", "aff4_bi", "geo"}
+    finally:
+        b200.b200_ctx_destroy(ctx)
+
+
+def test_work_lists_and_dmvr_deltas_in_arrays_that_start_in_a_registered_page(b200, oracle):
+    """b200_decompress_picture reads the PU list from, and b200_wait_picture writes the DMVR deltas into, host arrays that start in the last bytes of a page
+    the caller registered for another array and run past it (the layout the glue's pinned work-list vectors can give the decoder's own arrays): both
+    copies still move every byte."""
+    rng = np.random.default_rng(13)
+    W, H, bd = 416, 240, 10
+    g = abi.make_geom(W, H, bd)
+    dpb = [synth.noise_planes(rng, W, H, bd) for _ in range(4)]
+    pic = synth.gen_picture(rng, W, H, bd, dst_slot=4, deblock=False, sao=False, alf=False, pu_kw=dict(p_dmvr=0.9, p_bi=0.9, mv_sigma=2.0))
+    want, dm_want = oracle_decompress(oracle, g, dpb, pic)
+    assert (dm_want != 0).any() and len(dm_want) * 8 > 64
+    page = 4096
+    raw = np.zeros(2 * page + len(dm_want) * 8 + page, np.uint8)
+    base = (-raw.ctypes.data) % page
+    rawp = np.zeros(2 * page + pic["pus"].nbytes + page, np.uint8)
+    basep = (-rawp.ctypes.data) % page
+    assert b200.b200_host_register(raw.ctypes.data + base, page) == 0
+    assert b200.b200_host_register(rawp.ctypes.data + basep, page) == 0
+    pus = rawp[basep + page - 64:basep + page - 64 + pic["pus"].nbytes].view(synth.PU_DTYPE)
+    pus[:] = pic["pus"]; pic["struct"].pus = pus.ctypes.data
+    ctx = C.c_void_p()
+    try:
+        vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 2, -1))
+        for s in range(4): vvdec_b200.check(b200.b200_ctx_load_slot(ctx, s, abi.plane_ptrs(dpb[s])))
+        dm = raw[base + page - 64:base + page - 64 + dm_want.size * 4].view(np.int32).reshape(dm_want.shape)
+        h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"])); assert h >= 0, b200.b200_last_error()
+        vvdec_b200.check(b200.b200_wait_picture(ctx, h, dm.ctypes.data, len(dm)))
+        assert np.array_equal(dm, dm_want)
+        got = [np.zeros_like(p) for p in want]
+        vvdec_b200.check(b200.b200_get_frame(ctx, 4, abi.plane_ptrs(got)))
+        for c in range(3): assert np.array_equal(got[c], want[c]), f"plane {c}"
+    finally:
+        if ctx: b200.b200_ctx_destroy(ctx)
+        b200.b200_host_unregister(raw.ctypes.data + base); b200.b200_host_unregister(rawp.ctypes.data + basep)

@@ -295,6 +295,11 @@ B200_API int b200_mc_predict_wp(const b200_geom* g, int16_t* const dst[3], const
                                 const b200_pu* pus, size_t numPus, int32_t* dmvrMv, size_t numDmvr, const b200_wp* wp, int numWp)
 {
   B200_CHECK(g && dst && refs && (pus || !numPus), "b200_mc_predict: null argument");
+  // K2 predicts 4:0:0 and 4:2:0 only; any other format would upload three planes and leave chroma unwritten
+  B200_CHECK(g->chromaFormat == 0 || g->chromaFormat == 1, "b200_mc_predict: chromaFormat %d (only 0 = 4:0:0 and 1 = 4:2:0)", g->chromaFormat);
+  B200_CHECK(g->bitDepth >= 8 && g->bitDepth <= 12, "b200_mc_predict: bit depth %d (8..12)", g->bitDepth);
+  B200_CHECK(g->width > 0 && g->height > 0 && g->stride[0] >= g->width && (!g->chromaFormat || (g->stride[1] >= g->width / 2 && g->stride[2] >= g->width / 2)),
+             "b200_mc_predict: a plane stride is smaller than the plane's width");
   B200_CHECK(numSlots >= 1 && numSlots <= B200_MAX_SLOTS, "b200_mc_predict: numSlots %d", numSlots);
   B200_CHECK(numPus < (1u << 26), "b200_mc_predict: too many PUs");
   for (size_t i = 0; i < numPus; i++) {

@@ -26,7 +26,10 @@ __device__ __forceinline__ PuHead pu_head(const b200_pu* pus, int i, const PuLim
   PuHead r; r.w = p.w; r.h = p.h; r.flags = p.flags;
   const int s0 = p.refSlot[0], s1 = p.refSlot[1], numSlots = slotsBd & 0xff, bitDepth = (slotsBd >> 8) & 0xff, numWp = slotsBd >> 16;
   r.bi = s0 >= 0 && s1 >= 0;
-  r.ok = s0 < numSlots && s1 < numSlots && (s0 >= 0 || s1 >= 0) && r.w >= 4 && r.h >= 4 && r.w <= 128 && r.h <= 128 && !(r.w & 3) && !(r.h & 3);
+  // sides are multiples of 4 (CUs: powers of two; SbTMVP runs: multiples of 8) whose 16-sample tiles end in a 4, 8 or 16 piece: mc_tile maps threads to
+  // samples with tw - 1 masks and log2(tw) shifts, so a 12-sample piece (sides 12, 28, 44, ...) would filter wrong columns and store below the tile
+  r.ok = s0 < numSlots && s1 < numSlots && (s0 >= 0 || s1 >= 0) && r.w >= 4 && r.h >= 4 && r.w <= 128 && r.h <= 128 && !(r.w & 3) && !(r.h & 3) &&
+         (r.w & 15) != 12 && (r.h & 15) != 12;
   // the block must lie inside the picture on the 4x4 grid (kernels write every sample of it), DMVR deltas inside the output array
   if ((p.x & 3) || (p.y & 3) || p.x + r.w > lim.W || p.y + r.h > lim.H) r.ok = false;
   if ((r.flags & B200_PU_DMVR) && (unsigned long long)p.dmvrOff + (unsigned)(max(1, r.w >> 4) * max(1, r.h >> 4)) > lim.numDmvr) r.ok = false;

@@ -608,6 +608,7 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
     }
 #pragma unroll
     for (int j = 0; j < OPT; j++) {
+      if (OPT == 1 && sy >= th) break;                       // a 4x4 tile runs in the 32-thread launch of its class: threads 16..31 have no sample
       int16_t* d = P.dst[0] + (size_t)(by + sy + j) * P.dstStride[0] + bx + sx;
       if (MODE == 1 && geo) *d = (int16_t)LUMA_OUT(geo_blend(geo_weight(pu.bcwW1, gl2w, gl2h, tx0 + sx, ty0 + sy + j, 0), (int16_t)(pr[0][j] >> 6), (int16_t)(pr[NL - 1][j] >> 6), hr, pmax));
       else if (MODE <= 1 && we) *d = (int16_t)LUMA_OUT(BI ? wp_bi(we, 0, (int16_t)(pr[0][j] >> 6), (int16_t)(pr[NL - 1][j] >> 6), hr, pmax) : wp_uni(we, 0, (int16_t)(pr[0][j] >> 6), hr, pmax));

@@ -72,6 +72,10 @@ struct b200_ctx {
 
 extern "C" {
 
+static int copy2d_host(void* dst, size_t dpitch, const void* src, size_t spitch, size_t wBytes, size_t h, cudaMemcpyKind kind, cudaStream_t s);
+// a contiguous copy between caller memory and the device (see copy2d_host: the caller's array may start in a page registered for another array)
+static inline int copy_host(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t s) { return copy2d_host(dst, bytes, src, bytes, bytes, 1, kind, s); }
+
 B200_API int b200_ctx_create(b200_ctx** out, const b200_geom* g, int numSlots, int numArenas, int device)
 {
   B200_CHECK(out && g, "b200_ctx_create: null argument");
@@ -135,7 +139,7 @@ B200_API int b200_ctx_load_slot(b200_ctx* c, int slot, const int16_t* const plan
   B200_CHECK(c && planes && slot >= 0 && slot < c->numSlots, "b200_ctx_load_slot: bad argument");
   DevPlanes d = c->planes(c->slotBuf[slot]);
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++)
-    B200_CUDA(cudaMemcpyAsync(d.p[k], planes[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyHostToDevice, c->stream));
+    if (int rc = copy_host(d.p[k], planes[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyHostToDevice, c->stream)) return rc;
   B200_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -191,7 +195,7 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   char* base = A.buf.as<char>();
   cudaStream_t s = c->upStream;                                       // H2D on its own stream: overlaps the kernels of earlier pictures
   if (A.donePending) { B200_CUDA(cudaStreamWaitEvent(s, A.done, 0)); A.donePending = false; }   // kernels of the arena's previous picture
-  auto h2d = [&](size_t o, const void* src, size_t bytes) -> int { if (bytes) B200_CUDA(cudaMemcpyAsync(base + o, src, bytes, cudaMemcpyHostToDevice, s)); return 0; };
+  auto h2d = [&](size_t o, const void* src, size_t bytes) -> int { if (bytes) if (int rc = copy_host(base + o, src, bytes, cudaMemcpyHostToDevice, s)) return rc; return 0; };
   if (int rc = h2d(oPus, p->pus, p->numPus * sizeof(b200_pu))) return rc;
   if (int rc = h2d(oTus, p->tus, p->numTus * sizeof(b200_tu))) return rc;
   if (int rc = h2d(oCoef, p->coefs, p->numCoefs * 2)) return rc;
@@ -389,7 +393,7 @@ B200_API int b200_wait_picture(b200_ctx* c, int ai, int32_t* dmvrMv, size_t numD
   B200_CHECK(c, "b200_wait_picture: null context");
   if (dmvrMv && ai >= 0 && ai < c->numArenas && c->arenas[ai].dmvrMv) {
     const size_t n = numDmvr < c->arenas[ai].numDmvr ? numDmvr : c->arenas[ai].numDmvr;
-    B200_CUDA(cudaMemcpyAsync(dmvrMv, c->arenas[ai].dmvrMv, n * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (n) { if (int rc = copy_host(dmvrMv, c->arenas[ai].dmvrMv, n * 8, cudaMemcpyDeviceToHost, c->stream)) return rc; }
   }
   B200_CUDA(cudaStreamSynchronize(c->upStream));
   B200_CUDA(cudaStreamSynchronize(c->stream));
@@ -406,7 +410,7 @@ B200_API int b200_get_frame(b200_ctx* c, int slot, int16_t* const planes[3])
   B200_CHECK(c && planes && slot >= 0 && slot < c->numSlots, "b200_get_frame: bad argument");
   DevPlanes d = c->planes(c->slotBuf[slot]);
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++)
-    B200_CUDA(cudaMemcpyAsync(planes[k], d.p[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyDeviceToHost, c->stream));
+    if (int rc = copy_host(planes[k], d.p[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyDeviceToHost, c->stream)) return rc;
   B200_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -414,7 +418,7 @@ B200_API int b200_get_frame(b200_ctx* c, int slot, int16_t* const planes[3])
 // Picture buffers of the host decoder carry margins (stride > width): 2-D copies between the margin-less device planes and strided host planes.
 // The runtime classifies a host range by its first address.  cudaHostRegister pins whole pages, so a plane that starts on a page the caller registered for
 // another array (the glue pins its work-list vectors, which share the heap with the decoder's picture buffers) and runs past that registration is refused with
-// cudaErrorInvalidValue.  Such a plane goes through a pinned staging copy instead.
+// cudaErrorInvalidValue.  Such a plane, like any other caller array this file copies (copy_host), goes through a pinned staging copy instead.
 static int copy2d_host(void* dst, size_t dpitch, const void* src, size_t spitch, size_t wBytes, size_t h, cudaMemcpyKind kind, cudaStream_t s)
 {
   const cudaError_t e = cudaMemcpy2DAsync(dst, dpitch, src, spitch, wBytes, h, kind, s);
@@ -472,7 +476,7 @@ B200_API int b200_get_frame_async(b200_ctx* c, int slot, int16_t* const planes[3
   B200_CUDA(cudaEventRecord(c->finalEv, c->stream));                 // everything submitted so far (incl. this slot's picture) is final after this
   B200_CUDA(cudaStreamWaitEvent(c->copyStream, c->finalEv, 0));
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++)
-    B200_CUDA(cudaMemcpyAsync(planes[k], d.p[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyDeviceToHost, c->copyStream));
+    if (int rc = copy_host(planes[k], d.p[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;
   const int t = c->nextTicket; c->nextTicket = (c->nextTicket + 1) & 15;
   B200_CUDA(cudaEventRecord(c->ticketEv[t], c->copyStream));
@@ -527,7 +531,7 @@ B200_API int b200_get_frame_fmt_async(b200_ctx* c, int slot, int fmt, void* cons
   if (int rc = launch_pack(d, c->g, fmt, dst, c->copyStream)) return rc;                      // on the copy stream: the kernel stream runs on
   c->launches += nPl;
   B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;       // the picture buffer is free once it is packed
-  for (int k = 0; k < nPl; k++) B200_CUDA(cudaMemcpyAsync(planes[k], dst[k], bytes[k], cudaMemcpyDeviceToHost, c->copyStream));
+  for (int k = 0; k < nPl; k++) if (int rc = copy_host(planes[k], dst[k], bytes[k], cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   const int t = c->nextTicket; c->nextTicket = (c->nextTicket + 1) & 15;
   B200_CUDA(cudaEventRecord(c->ticketEv[t], c->copyStream));
   return t;
@@ -554,10 +558,10 @@ B200_API int b200_get_frame_grain_async(b200_ctx* c, int slot, int fmt, void* co
   if (int rc = c->grainTab.reserve(tabBytes)) return rc;
   if (int rc = c->grainStage[st].reserve(c->picBytes)) return rc;
   uint8_t* tb = c->grainTab.as<uint8_t>();
-  B200_CUDA(cudaMemcpyAsync(tb, fg->pattern, oS, cudaMemcpyHostToDevice, c->copyStream));
-  B200_CUDA(cudaMemcpyAsync(tb + oS, fg->sLUT, 768, cudaMemcpyHostToDevice, c->copyStream));
-  B200_CUDA(cudaMemcpyAsync(tb + oP, fg->pLUT, 768, cudaMemcpyHostToDevice, c->copyStream));
-  B200_CUDA(cudaMemcpyAsync(tb + oL, fg->lineSeeds, (size_t)nby * 4, cudaMemcpyHostToDevice, c->copyStream));
+  if (int rc = copy_host(tb, fg->pattern, oS, cudaMemcpyHostToDevice, c->copyStream)) return rc;
+  if (int rc = copy_host(tb + oS, fg->sLUT, 768, cudaMemcpyHostToDevice, c->copyStream)) return rc;
+  if (int rc = copy_host(tb + oP, fg->pLUT, 768, cudaMemcpyHostToDevice, c->copyStream)) return rc;
+  if (int rc = copy_host(tb + oL, fg->lineSeeds, (size_t)nby * 4, cudaMemcpyHostToDevice, c->copyStream)) return rc;
   const int buf = c->slotBuf[slot];
   DevPlanes src = c->planes(buf), gr = src;
   { uint8_t* b = c->grainStage[st].as<uint8_t>(); gr.p[0] = reinterpret_cast<int16_t*>(b); gr.p[1] = reinterpret_cast<int16_t*>(b + c->planeBytes[0]); gr.p[2] = reinterpret_cast<int16_t*>(b + c->planeBytes[0] + c->planeBytes[1]); }
@@ -568,7 +572,7 @@ B200_API int b200_get_frame_grain_async(b200_ctx* c, int slot, int fmt, void* co
   c->launches += 1 + nPl;
   B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;       // the picture buffer is free once the grained copy exists
   if (fmt == B200_OUT_16) {
-    for (int k = 0; k < nPl; k++) B200_CUDA(cudaMemcpyAsync(planes[k], gr.p[k], (size_t)g.stride[k] * (k ? g.height >> 1 : g.height) * 2, cudaMemcpyDeviceToHost, c->copyStream));
+    for (int k = 0; k < nPl; k++) if (int rc = copy_host(planes[k], gr.p[k], (size_t)g.stride[k] * (k ? g.height >> 1 : g.height) * 2, cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   } else {
     size_t bytes[3] = {0, 0, 0}, off[3] = {0, 0, 0}, total = 0;
     for (int k = 0; k < nPl; k++) { bytes[k] = b200_frame_bytes(&g, fmt, k); off[k] = total; total += (bytes[k] + 255) & ~(size_t)255; }
@@ -577,7 +581,7 @@ B200_API int b200_get_frame_grain_async(b200_ctx* c, int slot, int fmt, void* co
     uint8_t* dst[3]; for (int k = 0; k < 3; k++) dst[k] = c->outStage[st].as<uint8_t>() + off[k];
     if (int rc = launch_pack(gr, g, fmt, dst, c->copyStream)) return rc;
     c->launches += nPl;
-    for (int k = 0; k < nPl; k++) B200_CUDA(cudaMemcpyAsync(planes[k], dst[k], bytes[k], cudaMemcpyDeviceToHost, c->copyStream));
+    for (int k = 0; k < nPl; k++) if (int rc = copy_host(planes[k], dst[k], bytes[k], cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   }
   const int t = c->nextTicket; c->nextTicket = (c->nextTicket + 1) & 15;
   B200_CUDA(cudaEventRecord(c->ticketEv[t], c->copyStream));
@@ -600,7 +604,7 @@ B200_API int b200_frame_hash_async(b200_ctx* c, int slot, int method, uint8_t* d
   if (int rc = launch_hash(c->planes(buf), c->g, method, acc, dig, c->copyStream)) return rc;
   c->launches += (c->g.chromaFormat ? 3 : 1) + 1;
   B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;
-  B200_CUDA(cudaMemcpyAsync(digest, dig, 12, cudaMemcpyDeviceToHost, c->copyStream));
+  if (int rc = copy_host(digest, dig, 12, cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   B200_CUDA(cudaEventRecord(c->ticketEv[t], c->copyStream));
   return t;
 }

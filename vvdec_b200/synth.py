@@ -857,3 +857,451 @@ def intra_sweep(ctu=128, ctus_w=32):
 def intra_record_key(r):
     """(comp, w, h, mode, multiRefIdx, mip) of a record: the block identity intra_sweep_blocks() lists."""
     return (int(r["comp"]), 1 << int(r["log2w"]), 1 << int(r["log2h"]), int(r["mode"]), int(r["multiRefIdx"]), int(r["mip"]))
+
+
+# ---------------------------------------------------------------------------------------------------------------- designed K2 sweep
+# A fixed list of named K2 cases (tests/test_k2_*.py): every PU shape under every tool it allows, every 1/16 luma phase pair in each tile list, tiles whose
+# reference windows sit on the interior / boundary thresholds of k2_inter.cu, MVs at the clipMv bounds and at +-2^17, and reference content built so that
+# DMVR's search provably ends where the case says.  Nothing is drawn at random except the noise of the reference pictures, from a seed fixed per case.
+MC_SIZES = (4, 8, 16, 32, 64, 128)
+MC_AFFINE_TOOLS = tuple(f"aff{n}_{d}{p}" for n in (4, 6) for d in ("uni", "bi") for p in ("", "_prof"))
+MC_TOOLS = ("uni0", "uni1", "bi", "bcw-2", "bcw3", "bcw5", "bcw10", "bdof", "dmvr", "dmvr_bdof", "althpel") + MC_AFFINE_TOOLS + ("geo",)
+MC_WP_TOOLS = ("wp_uni0", "wp_uni1", "wp_bi", "wp_aff4_uni", "wp_aff6_bi_prof")
+MC_LISTS = [(m, k) for m in range(4) for k in range(4) if m < 2 or k >= 2]       # the 12 translational (mode, size class) lists; 16 = affine
+
+
+def mc_tool_legal(tool, w, h):
+    """The shapes VVC allows a tool at (bucket.cu pu_head and InterPrediction.cpp:1372-1420): no bi-prediction for 4x4, 4x8 and 8x4; BCW from 256
+    samples; BDOF / DMVR from 8x8 and 128 samples; affine from 8x8; GEO 8..64 per side with an aspect ratio of at most 4.  A CU 128 samples wide or
+    high is at least 64 samples in the other direction (the 64x64 pipeline units forbid splitting a 128x64 CU further across its long side)."""
+    if max(w, h) == 128 and min(w, h) < 64: return False
+    big = w >= 8 and h >= 8 and w * h >= 128
+    t = tool[3:] if tool.startswith("wp_") else tool
+    if t in ("uni0", "uni1", "althpel"): return True
+    if t == "bi": return w + h > 12
+    if t.startswith("bcw"): return w * h >= 256
+    if t in ("bdof", "dmvr", "dmvr_bdof"): return big
+    if t.startswith("aff"): return w >= 8 and h >= 8
+    if t == "geo": return 8 <= w <= 64 and 8 <= h <= 64 and w < 8 * h and h < 8 * w
+    raise ValueError(tool)
+
+
+def mc_list_of(pu, tx, ty):
+    """bucket.cu mc_list_of: the list of luma tile (tx, ty) of a PU, mode * 4 + size class (32 / 64 / 128 / 256 samples), 16 = affine."""
+    f, w, h = int(pu["flags"]), int(pu["w"]), int(pu["h"])
+    if f & PU_AFFINE: return 16
+    bi = pu["refSlot"][0] >= 0 and pu["refSlot"][1] >= 0
+    mode = 1 if f & PU_GEO else 3 if f & PU_DMVR else 2 if bi and f & PU_BDOF else 1 if bi else 0
+    n = min(16, w - 16 * tx) * min(16, h - 16 * ty)
+    return mode * 4 + (0 if n <= 32 else 1 if n <= 64 else 2 if n <= 128 else 3)
+
+
+def mc_tiles(pus):
+    """Every luma tile of a PU list: (PU index, tx, ty, list)."""
+    return [(i, tx, ty, mc_list_of(p, tx, ty)) for i, p in enumerate(pus) for ty in range((int(p["h"]) + 15) // 16) for tx in range((int(p["w"]) + 15) // 16)]
+
+
+def mc_affine_over(pu, l):
+    """k2_inter.cu spread_over_limit / aff_model for list l of an affine PU (InterPrediction.cpp:1001-1030): the sub-block MVs collapse to the
+    centre MV and PROF is off when the spread of the 4x4 sub-block footprint is over the memory-bandwidth limit."""
+    l2w, l2h = int(pu["w"]).bit_length() - 1, int(pu["h"]).bit_length() - 1
+    LT, RT, LB = [int(v) for v in pu["mv"][l]], [int(v) for v in pu["cpmv"][l][0]], [int(v) for v in pu["cpmv"][l][1]]
+    a, b = (RT[0] - LT[0]) << (7 - l2w), (RT[1] - LT[1]) << (7 - l2w)
+    if pu["flags"] & PU_AFFINE6: c, d = (LB[0] - LT[0]) << (7 - l2h), (LB[1] - LT[1]) << (7 - l2h)
+    else: c, d = -b, a
+    s4, ft = 4 << 11, 6
+    if pu["interDir"] == 3:
+        xs, ys = (0, 4 * a + s4, 4 * c, 4 * a + 4 * c + s4), (0, 4 * b, 4 * d + s4, 4 * b + 4 * d + s4)
+        return (((max(xs) - min(xs)) >> 11) + ft + 3) * (((max(ys) - min(ys)) >> 11) + ft + 3) > (ft + 9) * (ft + 9)
+    rw, rh = ((max(0, 4 * a + s4) - min(0, 4 * a + s4)) >> 11) + ft + 3, ((max(0, 4 * b) - min(0, 4 * b)) >> 11) + ft + 3
+    if rw * rh > (ft + 9) * (ft + 5): return True
+    rw, rh = ((max(0, 4 * c) - min(0, 4 * c)) >> 11) + ft + 3, ((max(0, 4 * d + s4) - min(0, 4 * d + s4)) >> 11) + ft + 3
+    return rw * rh > (ft + 5) * (ft + 9)
+
+
+def _mc_pu(x, y, w, h, slots, mv0=(0, 0), mv1=(0, 0), flags=0, bcw=4, cpmv=None):
+    r = np.zeros((), PU_DTYPE)
+    r["x"], r["y"], r["w"], r["h"], r["flags"], r["bcwW1"] = x, y, w, h, flags, bcw
+    r["refSlot"] = slots
+    r["interDir"] = 3 if slots[0] >= 0 and slots[1] >= 0 else 1 if slots[0] >= 0 else 2
+    r["mv"] = (mv0, mv1)
+    if cpmv is not None: r["cpmv"] = cpmv
+    return r
+
+
+def _mc_mv(k, salt=0):
+    """MV number k of a cycle: phase pair (k * 7 + salt) mod 256 of the 16 x 16 luma phases, and with it both values of the extra chroma phase bit
+    (so every 1/32 chroma phase), integer part -4..4 / -3..3 samples."""
+    i = (k * 7 + salt) % 256
+    fx, fy = i % 16, i // 16
+    ax, ay = (k * 5 + salt) % 9 - 4, (k * 3 + salt) % 7 - 3
+    return (ax * 32 + ((i >> 4) & 1) * 16 + fx, ay * 32 + (i & 1) * 16 + fy)
+
+
+def _mc_tool_pu(tool, x, y, w, h, k):
+    """The PU of `tool` at (x, y, w, h), k-th of its kind (k cycles the phases, the reference slots and the affine / GEO parameters)."""
+    mv0, mv1 = _mc_mv(k), _mc_mv(k, 101)
+    p = k & 1
+    t = tool[3:] if tool.startswith("wp_") else tool
+    if t == "uni0": return _mc_pu(x, y, w, h, (p, -1), mv0)
+    if t == "uni1": return _mc_pu(x, y, w, h, (-1, 2 + p), mv0, mv1)
+    if t in ("bi", "bi_small"): return _mc_pu(x, y, w, h, (p, 2 + ((k >> 1) & 1)), mv0, mv1)
+    if t.startswith("bcw"): return _mc_pu(x, y, w, h, (p, 2 + ((k >> 1) & 1)), mv0, mv1, bcw=int(t[3:]))
+    if t == "bdof": return _mc_pu(x, y, w, h, (p, 2 + p), mv0, mv1, PU_BDOF)
+    if t in ("dmvr", "dmvr_bdof"): return _mc_pu(x, y, w, h, (p, 2 + p), mv0, mv1, PU_DMVR | (PU_BDOF if t == "dmvr_bdof" else 0))
+    if t == "althpel":                                          # AMVR half-pel: MVs in half samples, the 6-tap half-sample filter; chroma 0, 8, 16, 24 / 32
+        a0, a1 = (8 * ((k % 4) - 2), 8 * ((k // 4) % 4 - 2)), (8 * ((k * 3) % 8 - 4), 8 * ((k * 5 + 1) % 8 - 3))
+        return _mc_pu(x, y, w, h, (p, 2 + p) if w + h > 12 else (p, -1), a0, a1, PU_ALTHPEL)
+    if t.startswith("aff"):
+        six, bi, prof = t.startswith("aff6"), "_bi" in t, t.endswith("_prof")
+        d = [(((k * 13 + 7 * l) % 49) - 24, ((k * 29 + 3 * l) % 49) - 24) for l in range(4)]
+        cp = [[(mv0[0] + d[0][0], mv0[1] + d[0][1]), (mv0[0] + d[1][0], mv0[1] + d[1][1])], [(mv1[0] + d[2][0], mv1[1] + d[2][1]), (mv1[0] + d[3][0], mv1[1] + d[3][1])]]
+        fl = PU_AFFINE | (PU_AFFINE6 if six else 0) | (PU_PROF0 | PU_PROF1 if prof else 0)
+        return _mc_pu(x, y, w, h, (p, 2 + p) if bi else ((p, -1) if k & 2 else (-1, 2 + p)), mv0, mv1, fl, cpmv=cp)
+    if t == "geo": return _mc_pu(x, y, w, h, (k % 4, (k * 3 + 1) % 4), mv0, mv1, PU_GEO, bcw=k % 64)
+    raise ValueError(tool)
+
+
+def _mc_pack(sizes, W, gap=0, margin=0):
+    """Shelf packing of (w, h) rectangles (powers of two) into a picture W wide, tallest first.  Every block starts at a multiple of its own size, so no
+    block crosses a CTU boundary (a CU never does; the reference keeps motion per CTU).  Returns (positions, height used)."""
+    order = sorted(range(len(sizes)), key=lambda i: (-sizes[i][1], -sizes[i][0], i))
+    up = lambda v, a: (v + a - 1) // a * a
+    pos = [None] * len(sizes); x = margin; y = margin; rowh = 0
+    for i in order:
+        w, h = sizes[i]
+        if up(x, w) + w > W - margin or rowh == 0:
+            y = up(y + rowh + (gap if rowh else 0), h); x = margin; rowh = h
+        x = up(x, w)
+        pos[i] = (x, y); x += w + gap
+    return pos, y + rowh + margin
+
+
+def _mc_finish(pus):
+    """dmvrOff of the DMVR PUs (one entry per 16x16 sub-block), the list as an array, the number of entries."""
+    pus = np.array(pus, PU_DTYPE)
+    off = 0
+    for p in pus:
+        if p["flags"] & PU_DMVR:
+            p["dmvrOff"] = off; off += max(1, int(p["w"]) >> 4) * max(1, int(p["h"]) >> 4)
+    return pus, off
+
+
+def mc_shape_tool_specs(tools=MC_TOOLS, bd=10):
+    """(tool, w, h) of every legal shape x tool pair (DMVR only up to 10 bit); GEO: the 64 split directions spread over its 14 shapes; plus the bi-predicted
+    4x8 / 8x4 blocks ('bi_small'): the standard never codes them, but the PU list accepts them and they are what fills the 32-sample bi list."""
+    out = []
+    for t in tools:
+        if t.endswith("geo"): continue
+        if bd > 10 and "dmvr" in t: continue
+        out += [(t, w, h) for h in MC_SIZES for w in MC_SIZES if mc_tool_legal(t, w, h)]
+    if "geo" in tools:
+        shapes = [(w, h) for h in MC_SIZES for w in MC_SIZES if mc_tool_legal("geo", w, h)]
+        out += [("geo", *shapes[d % len(shapes)]) for d in range(64)]
+        out += [("bi_small", 8, 4), ("bi_small", 4, 8)]
+    return out
+
+
+def _mc_shapes_case(W, specs, gap=0, ctu=128):
+    """The PUs of (tool, w, h) specs no larger than the CTU, packed into a picture W wide, the k-th of each tool with the k-th MV of its cycle."""
+    specs = [s for s in specs if max(s[1], s[2]) <= ctu]
+    pos, used = _mc_pack([(w, h) for _, w, h in specs], W, gap=gap)
+    count, pus, tags = {}, [], []
+    for (t, w, h), (x, y) in zip(specs, pos):
+        k = count.get(t, 0); count[t] = k + 1
+        pus.append(_mc_tool_pu(t, x, y, w, h, k)); tags.append(t)
+    return pus, tags, used
+
+
+def _mc_phase_case(W):
+    """256 single-tile PUs per translational list, one per luma phase pair of list 0 (list 1 cycles independently), + AltHpel PUs of every class."""
+    shape = {0: (8, 4), 1: (8, 8), 2: (16, 8), 3: (16, 16)}
+    tool = {0: "uni0", 1: "bi", 2: "bdof", 3: "dmvr"}
+    specs = []
+    for (m, c) in MC_LISTS:
+        t = "bi_small" if (m, c) == (1, 0) else tool[m]
+        specs += [(t, *shape[c], (m, c), k) for k in range(256)]
+    specs += [("althpel", *shape[c], None, k) for c in range(4) for k in range(16)]
+    pos, used = _mc_pack([(w, h) for _, w, h, _, _ in specs], W)
+    pus, tags = [], []
+    for (t, w, h, lst, k), (x, y) in zip(specs, pos):
+        pu = _mc_tool_pu(t, x, y, w, h, k)
+        if lst is not None:                                    # phase pair k exactly (the integer part still cycles)
+            mv = _mc_mv(k); fx, fy = k % 16, k // 16
+            pu["mv"][0] = ((mv[0] & ~15) | fx, (mv[1] & ~15) | fy)
+        pus.append(pu); tags.append(t)
+    return pus, tags, used
+
+
+# ---- windows of a tile (k2_inter.cu): the integer reference position of its first sample, and the interior tests
+def mc_tile_windows(pu, l, tx=0, ty=0):
+    """Integer reference positions of tile (tx, ty) of a PU for list l before any clipping: luma (ox, oy), chroma (ocx, ocy) as the uni / bi / BDOF tiles
+    compute them, and the DMVR search origins (ix, iy), (icx, icy) (mc_tile, :275 and :458)."""
+    bx, by = int(pu["x"]) + 16 * tx, int(pu["y"]) + 16 * ty
+    mx, my = int(pu["mv"][l][0]), int(pu["mv"][l][1])
+    return dict(luma=(bx + (mx >> 4), by + (my >> 4)), chroma=((bx >> 1) + (mx >> 5), (by >> 1) + (my >> 5)),
+                dmvr=(bx + (mx >> 4), by + (my >> 4)), dmvr_chroma=((bx >> 1) + (mx >> 5), (by >> 1) + (my >> 5)))
+
+
+def mc_window_margins(kind, W, H, tw, th):
+    """For a window kind, (first interior x, last interior x, first interior y, last interior y) of its origin: k2_inter.cu :472-473 (luma / chroma
+    footprints of the 8- / 4-tap filters) and :276-277 (DMVR search windows)."""
+    cw, ch, CW, CH = tw >> 1, th >> 1, W >> 1, H >> 1
+    if kind == "luma": return 4, W - tw - 5, 3, H - th - 4
+    if kind == "chroma": return 2, CW - cw - 3, 1, CH - ch - 2
+    if kind == "dmvr": return 6, W - tw - 9, 6, H - th - 9
+    if kind == "dmvr_chroma": return 4, CW - cw - 6, 3, CH - ch - 5
+    raise ValueError(kind)
+
+
+def _mc_edge_specs(chroma, bd):
+    """Single-tile PUs of one shape per translational list x window kind x edge x offset (-1, 0, +1 around the first interior position)."""
+    shape = {(0, 0): (8, 4), (0, 1): (8, 8), (0, 2): (16, 8), (0, 3): (16, 16), (1, 0): (4, 8), (1, 1): (8, 8), (1, 2): (8, 16), (1, 3): (16, 16),
+             (2, 2): (16, 8), (2, 3): (16, 16), (3, 2): (8, 16), (3, 3): (16, 16)}
+    tool = {0: "uni0", 1: "bi", 2: "bdof", 3: "dmvr_bdof"}
+    out = []
+    for (m, c) in MC_LISTS:
+        if m == 3 and bd > 10: continue
+        kinds = ("dmvr",) + (("dmvr_chroma",) if chroma else ()) if m == 3 else ("luma",) + (("chroma",) if chroma else ())
+        for kind in kinds:
+            for edge in "lrtb":
+                for off in (-1, 0, 1):
+                    out.append(("bi_small" if (m, c) == (1, 0) else tool[m], *shape[(m, c)], kind, edge, off))
+    return out
+
+
+def _mc_edges_case(W, H, ctu, chroma, bd):
+    """Threshold tiles (see _mc_edge_specs), PUs with MVs at the clipMv bounds of this CTU size and one sample past them, and MVs near +-2^17.  The
+    affine ones among the latter have sub-block MVs past the +-2^17 storage clamp.  The DMVR ones do not make the refinement cross that clamp
+    (k2_inter.cu :409): both search windows lie wholly outside the picture, where every sample replicates the border, so the search ends at the centre
+    with a zero delta.  No picture narrower than 2^13 samples can do otherwise, and clipMv follows the clamp in any case."""
+    specs = _mc_edge_specs(chroma, bd)
+    tools = ("uni0", "bi", "aff4_uni_prof") + (("dmvr_bdof",) if bd <= 10 else ())
+    bounds = ("xlo", "xlo-1", "xhi", "xhi+1", "ylo", "ylo-1", "yhi", "yhi+1")
+    clip = [(tools[(i + j) % len(tools)], s, s, b) for i, b in enumerate(bounds) for j, s in enumerate((32, 64, 128) if i % 2 == 0 else (32, 64)) if s <= ctu]
+    far = [(t, 16, 16, s) for t in ("uni0", "bi", "aff4_bi", "aff6_uni_prof") + (("dmvr", "dmvr_bdof") if bd <= 10 else ()) for s in (1, -1)]
+    sizes = [(w, h) for _, w, h, *_ in specs] + [(w, h) for _, w, h, _ in clip] + [(w, h) for _, w, h, _ in far]
+    pos, used = _mc_pack(sizes, W)
+    assert used <= H, (used, H)
+    pus, tags, marks = [], [], []
+    for k, ((t, w, h, kind, edge, off), (x, y)) in enumerate(zip(specs, pos)):
+        pu = _mc_tool_pu(t, x, y, w, h, k)
+        bi = pu["refSlot"][0] >= 0 and pu["refSlot"][1] >= 0
+        l = (k & 1) if bi else 0                               # the list that sits on the threshold; the other one looks at the centre
+        x0, x1, y0, y1 = mc_window_margins(kind, W, H, w, h)
+        sh = 5 if kind in ("chroma", "dmvr_chroma") else 4
+        bx, by = (x >> 1, y >> 1) if sh == 5 else (x, y)
+        tx_, ty_ = (x0 + x1) // 2, (y0 + y1) // 2
+        if edge == "l": tx_ = x0 + off
+        if edge == "r": tx_ = x1 + off
+        if edge == "t": ty_ = y0 + off
+        if edge == "b": ty_ = y1 + off
+        f = int(pu["mv"][l][0]) & ((1 << sh) - 1), int(pu["mv"][l][1]) & ((1 << sh) - 1)
+        pu["mv"][l] = (((tx_ - bx) << sh) + f[0], ((ty_ - by) << sh) + f[1])
+        if bi:
+            o = 1 - l; cx, cy = W // 2 - w // 2, H // 2 - h // 2
+            pu["mv"][o] = (((cx - x) << 4) + (int(pu["mv"][o][0]) & 15), ((cy - y) << 4) + (int(pu["mv"][o][1]) & 15))
+        pus.append(pu); tags.append(t); marks.append((len(pus) - 1, kind, edge, off, l))
+    n0 = len(specs)
+    for k, ((t, w, h, b), (x, y)) in enumerate(zip(clip, pos[n0:n0 + len(clip)])):
+        pu = _mc_tool_pu(t, x, y, w, h, k)
+        lo = lambda p: (-ctu - 8 - p + 1) * 16
+        hi = lambda p, S: (S + 8 - p - 1) * 16
+        v = {"xlo": lo(x), "xlo-1": lo(x) - 16, "xhi": hi(x, W), "xhi+1": hi(x, W) + 16,
+             "ylo": lo(y), "ylo-1": lo(y) - 16, "yhi": hi(y, H), "yhi+1": hi(y, H) + 16}[b] + (k % 5) * 3
+        for l in range(2):
+            mv = [int(pu["mv"][l][0]), int(pu["mv"][l][1])]
+            mv[0 if b[0] == "x" else 1] = v
+            if t.startswith("aff"): pu["cpmv"][l] = pu["cpmv"][l] - pu["mv"][l] + mv
+            pu["mv"][l] = mv
+        pus.append(pu); tags.append(t); marks.append((len(pus) - 1, "clip", b, 0, 0))
+    n1 = n0 + len(clip)
+    for k, ((t, w, h, s), (x, y)) in enumerate(zip(far, pos[n1:])):
+        pu = _mc_tool_pu(t, x, y, w, h, k)
+        m = (1 << 17) - 1
+        mv0, mv1 = (s * m - s * 9, -s * m + s * 12), (-s * m + s * 7, s * m - s * 20)
+        if t.startswith("aff"): pu["cpmv"] = [[(mv0[0] + 400 * s, mv0[1]), (mv0[0], mv0[1] + 300 * s)], [(mv1[0] - 400 * s, mv1[1] + 200), (mv1[0], mv1[1] - 300 * s)]]
+        pu["mv"] = (mv0, mv1)
+        pus.append(pu); tags.append(t); marks.append((len(pus) - 1, "far", "+" if s > 0 else "-", 0, 0))
+    return pus, tags, marks
+
+
+def _mc_affine_case(W, ctu):
+    """Affine PUs with CPMV spreads one step under and one step over the bandwidth limit (4- / 6-parameter, uni / bi, PROF on), equal CPMVs (PROF off
+    whatever the flag says), in every affine size class."""
+    specs = []
+    for (w, h) in ((8, 8), (16, 16), (32, 16), (16, 64), (64, 64), (128, 64)):
+        for six in (0, 1):
+            for bi in (0, 1):
+                for side in ("under", "over", "equal"):
+                    if max(w, h) <= ctu: specs.append((w, h, six, bi, side, (len(specs) // 3) & 1))
+    pos, used = _mc_pack([(w, h) for w, h, *_ in specs], W)
+    pus, tags = [], []
+    for k, ((w, h, six, bi, side, dirn), (x, y)) in enumerate(zip(specs, pos)):
+        t = f"aff{6 if six else 4}_{'bi' if bi else 'uni'}_prof"
+        pu = _mc_tool_pu(t, x, y, w, h, k)
+        for l in range(2):
+            base = np.array(pu["mv"][l], np.int64)
+            if side == "equal":
+                pu["cpmv"][l] = (base, base); continue
+            step = 0
+            def with_step(s):
+                q = pu.copy()
+                d = (s, 0) if dirn == 0 else (0, s)
+                q["cpmv"][l] = (base + d, base + ((0, s) if six and dirn == 0 else (s, 0) if six else (0, 0)))
+                return q
+            while not mc_affine_over(with_step(step + 1), l) and step < 4000: step += 1
+            pu["cpmv"][l] = with_step(step + (1 if side == "over" else 0))["cpmv"][l]
+        pus.append(pu); tags.append(t)
+    return pus, tags, used
+
+
+def _mc_dmvr_target_case(W):
+    """DMVR PUs whose mirrored search provably ends on a chosen one of the 25 integer positions: slots 2 / 3 are copies of slots 0 / 1 (slot 3 shifted by
+    (3, -2) samples), so that list 1's MV is list 0's + 2 * target - shift and the SAD is zero exactly there.  Centre targets stand for the early exit."""
+    shapes = [(16, 16), (8, 16), (16, 8), (32, 16), (16, 32), (64, 64)]
+    specs = [(d, shapes[(d + j) % len(shapes)], j) for d in range(25) for j in range(3)] + [(d, (128, 128), 0) for d in (3, 21)]
+    pos, used = _mc_pack([s for _, s, _ in specs], W, gap=4, margin=32)
+    pus, tags, targets = [], [], []
+    for k, ((d, (w, h), j), (x, y)) in enumerate(zip(specs, pos)):
+        u, v = d % 5 - 2, d // 5 - 2
+        p = k & 1
+        s = (0, 0) if p == 0 else (3, -2)
+        mv0 = _mc_mv(k); mv0 = ((mv0[0] & 15) + 16 * ((k % 5) - 2), (mv0[1] & 15) + 16 * ((k % 3) - 1))
+        mv1 = (mv0[0] + 16 * (2 * u - s[0]), mv0[1] + 16 * (2 * v - s[1]))
+        pus.append(_mc_pu(x, y, w, h, (p, 2 + p), mv0, mv1, PU_DMVR | (PU_BDOF if j != 1 else 0))); tags.append("dmvr_target")
+        targets.append((len(pus) - 1, u, v))
+    return pus, tags, targets, used
+
+
+# designed DMVR cost surfaces (content along x or y only, integer MVs): name -> (pattern, expected delta); see _mc_paint
+MC_DMVR_SURFACES = {
+    "tie_minus8_x": (-8, 0), "tie_plus8_x": (8, 0), "tie_minus8_y": (0, -8), "tie_plus8_y": (0, 8),     # a neighbour's SAD equals the scaled centre cost
+    "den0_x": (0, 0), "den0_y": (0, 0),                                                                  # both neighbours equal it: the surface is flat
+    "den0_x_bio_off": (0, 0),                                                                            # the same with minCost in [tw*th, 2*tw*th): BDOF off
+    "den0_x_ramp_y_bio_off": (0, 5),       # + a vertical ramp of 3 per row in both lists: the y surface is no longer flat, and BDOF would change samples
+    "flat_exit": (0, 0),                                                                                 # identical flat windows: SAD 0, the early exit
+}
+
+
+def _mc_paint(kind, A, B, x0, y0, w, h):
+    """Paints the windows of a PU at (x0, y0) in slot planes A (list 0) and B (list 1), 8 samples beyond the block on every side.
+    tie_*: A is a ramp of slope 7, B = A -+ 8, so that the SAD of shift u is N |14u +- 8|: u = -+1 costs 6N = the centre's 8N scaled by 3/4, and the strict
+    raster-order search keeps the centre, with an equal neighbour.  den0_*: A has period 4 (0 0 K K), B = A shifted by 2 plus c = 3K/4: odd shifts cost
+    c N = 3/4 of the centre's K N, even ones K N."""
+    ys, xs = np.mgrid[y0 - 8:y0 + h + 8, x0 - 8:x0 + w + 8]
+    axis = xs - (x0 - 8) if kind.endswith("_x") or "_x_" in kind else ys - (y0 - 8)
+    sl = (slice(y0 - 8, y0 + h + 8), slice(x0 - 8, x0 + w + 8))
+    if kind.startswith("tie"):
+        a = 16 + 7 * axis
+        A[sl] = a; B[sl] = a - 8 if "minus" in kind else a + 8
+    elif kind.startswith("den0"):
+        K, c = (4, 3) if kind.endswith("bio_off") else (40, 30)
+        ramp = 3 * (ys - (y0 - 8)) if "ramp_y" in kind else 0
+        A[sl] = 300 + K * ((axis % 4) >= 2) + ramp; B[sl] = 300 + K * (((axis + 2) % 4) >= 2) + c + ramp
+    elif kind == "flat_exit":
+        A[sl] = 77; B[sl] = 77
+
+
+def _mc_surface_case(W):
+    shapes = [(16, 16), (8, 16), (16, 8), (32, 32), (32, 16)]
+    specs = [(kind, s, bdof) for kind in MC_DMVR_SURFACES for s in shapes for bdof in (0, 1)]
+    pos, used = _mc_pack([s for _, s, _ in specs], W, gap=24, margin=16)
+    pus, tags = [], []
+    for (kind, (w, h), bdof), (x, y) in zip(specs, pos):
+        pus.append(_mc_pu(x, y, w, h, (0, 2), (0, 0), (0, 0), PU_DMVR | (PU_BDOF if bdof else 0))); tags.append(kind)
+    return pus, tags, used
+
+
+def _mc_refs(name, W, H, bd, chroma, strides, recipe, pus=None, tags=None):
+    """The four DPB slots of a case.  recipe: 'noise' (independent noise per slot), 'copies' (slots 2 / 3 = slots 0 / 1, slot 3 rolled by (3, -2)),
+    'flat' (one value per slot, slots 0 and 2 equal), 'extreme' (0 / 2^bd-1 checkerboards, stripes and steps), 'surfaces' (painted DMVR cost surfaces)."""
+    import zlib
+    rng = np.random.default_rng(zlib.crc32(name.encode()))
+    pmax = (1 << bd) - 1
+    slots = [noise_planes(rng, W, H, bd, chroma=chroma, strides=strides) for _ in range(4)]
+    if recipe == "copies":
+        slots[2] = [p.copy() for p in slots[0]]
+        slots[3] = []
+        for c, p in enumerate(slots[1]):
+            w = W >> (1 if c else 0); q = p.copy()
+            q[:, :w] = np.roll(p[:, :w], (2 >> (1 if c else 0), -3 >> (1 if c else 0)), axis=(0, 1))
+            slots[3].append(q)
+    elif recipe in ("flat", "surfaces"):
+        vals = (bd > 8 and 700 or 180, 300 >> (10 - bd) if bd <= 10 else 1200, bd > 8 and 700 or 180, 5)
+        for s in range(4):
+            for p in slots[s]: p[...] = vals[s]
+    elif recipe == "extreme":
+        for s in range(4):
+            for c, p in enumerate(slots[s]):
+                h, w = p.shape[0], W >> (1 if c else 0)
+                yy, xx = np.mgrid[0:h, 0:w]
+                pat = [((xx + yy) & 1), ((xx // 3) & 1), ((yy // 2) & 1) ^ ((xx // 5) & 1), (xx >= w // 2 + ((yy * 3) % 7) - 3)][s]
+                p[:, :w] = np.where(pat, pmax, 0)
+    if recipe == "surfaces":
+        for pu, kind in zip(pus, tags):
+            _mc_paint(kind, slots[0][0], slots[2][0], int(pu["x"]), int(pu["y"]), int(pu["w"]), int(pu["h"]))
+    if not chroma:
+        slots = [[s[0], s[0][:1], s[0][:1]] for s in slots]
+    return slots
+
+
+# name -> (W, H, bitDepth, CTU size, 4:2:0?, strides or None, content of the slots, builder)
+MC_SWEEP_CASES = {
+    "shapes_10bit": (1920, 1080, 10, 128, 1, None, "noise", "shapes"),
+    "shapes_8bit_extreme": (1920, 1080, 8, 128, 1, None, "extreme", "shapes"),
+    "shapes_12bit_extreme": (1920, 1080, 12, 128, 1, None, "extreme", "shapes"),
+    "shapes_10bit_flat": (1920, 1080, 10, 128, 1, None, "flat", "shapes"),
+    "shapes_yuv400_10bit": (1920, 1080, 10, 128, 0, None, "noise", "shapes"),
+    "phases_10bit": (1920, 400, 10, 128, 1, None, "noise", "phases"),
+    "phases_8bit_stride_odd": (1920, 400, 8, 64, 1, (1923, 961, 961), "noise", "phases"),
+    "edges_ctu128": (832, 480, 10, 128, 1, None, "noise", "edges"),
+    "edges_ctu64_stride_pad": (832, 472, 10, 64, 1, (836, 418, 418), "noise", "edges"),
+    "edges_ctu32_stride_odd": (832, 480, 10, 32, 1, (833, 417, 417), "noise", "edges"),
+    "edges_ctu32_yuv400_8bit": (832, 456, 8, 32, 0, None, "noise", "edges"),
+    "edges_ctu64_12bit_extreme": (832, 472, 12, 64, 1, (840, 420, 420), "extreme", "edges"),
+    "affine_limits_10bit": (832, 480, 10, 128, 1, None, "noise", "affine"),
+    "affine_limits_12bit_stride_odd": (832, 480, 12, 64, 1, (833, 417, 417), "extreme", "affine"),
+    "dmvr_targets_10bit": (1280, 720, 10, 128, 1, None, "copies", "targets"),
+    "dmvr_targets_8bit_stride_pad": (1280, 720, 8, 128, 1, (1284, 642, 642), "copies", "targets"),
+    "dmvr_surfaces_10bit": (1280, 720, 10, 128, 1, None, "surfaces", "surfaces"),
+    "wp_10bit": (1920, 1080, 10, 128, 1, None, "noise", "wp"),
+    "wp_12bit_extreme": (1920, 1080, 12, 128, 1, None, "extreme", "wp"),
+    "wp_8bit_stride_odd": (1920, 1080, 8, 128, 1, (1921, 961, 961), "noise", "wp"),
+}
+
+_mc_sweep_cache = {}
+
+
+def mc_sweep(name):
+    """One case of the designed K2 sweep (MC_SWEEP_CASES) as a dict: geometry (g, W, H, bd, ctu, chroma, strides), the PU list and its number of DMVR
+    entries, the DPB slots (refs), the tool / pattern of every PU (tags), explicit weights (wp = (raw, entries)) for the wp cases, threshold marks
+    (edges cases: (PU index, window kind, edge, offset, list)) and DMVR targets ((PU index, u, v) for the targets case)."""
+    if name in _mc_sweep_cache: return _mc_sweep_cache[name]
+    from . import abi as A
+    W, H, bd, ctu, chroma, strides, recipe, kind = MC_SWEEP_CASES[name]
+    marks, targets, wp = [], [], None
+    if kind == "shapes":
+        pus, tags, used = _mc_shapes_case(W, mc_shape_tool_specs(bd=bd), ctu=ctu)
+    elif kind == "wp":
+        pus, tags, used = _mc_shapes_case(W, mc_shape_tool_specs(MC_WP_TOOLS + ("bcw3", "bcw-2", "geo"), bd), ctu=ctu)
+    elif kind == "phases":
+        pus, tags, used = _mc_phase_case(W)
+    elif kind == "edges":
+        pus, tags, marks = _mc_edges_case(W, H, ctu, chroma, bd); used = 0
+    elif kind == "affine":
+        pus, tags, used = _mc_affine_case(W, ctu)
+    elif kind == "targets":
+        pus, tags, targets, used = _mc_dmvr_target_case(W)
+    elif kind == "surfaces":
+        pus, tags, used = _mc_surface_case(W)
+    assert used <= H, (name, used, H)
+    pus, ndmvr = _mc_finish(pus)
+    if kind == "wp":
+        wp = gen_wp(np.random.default_rng(bd), bd, pus)
+    refs = _mc_refs(name, W, H, bd, bool(chroma), strides, recipe, pus, tags)
+    g = A.make_geom(W, H, bd, chroma_format=chroma, ctu=ctu, strides=strides or ((W, W >> 1, W >> 1) if chroma else (W, 0, 0)))
+    case = dict(name=name, g=g, W=W, H=H, bd=bd, ctu=ctu, chroma=chroma, strides=(g.stride[0], g.stride[1], g.stride[2]), pus=pus, ndmvr=ndmvr, refs=refs,
+                tags=tags, marks=marks, targets=targets, wp=wp)
+    _mc_sweep_cache[name] = case
+    return case
