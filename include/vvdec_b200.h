@@ -126,8 +126,20 @@ typedef struct b200_lf_seq {        /* SPS luma-adaptive deblocking (LADF), Slic
   int32_t ladfIntervalLowerBound[5];
 } b200_lf_seq;
 
-/* Kernel-level K3 on host planes (in place). lfV/lfH: [ceil(H/4)][ceil(W/4)] rasters. ctuSlice: slice index of
- * every CTU in raster order (NULL: all slice 0). seq may be NULL (LADF off). dirs: bit0 = vertical edges, bit1 = horizontal. */
+/* Kernel-level K3 on host planes (in place). lfV/lfH: [H/4][W/4] rasters. ctuSlice: slice index of
+ * every CTU in raster order (NULL: all slice 0). seq may be NULL (LADF off). dirs: bit0 = vertical edges, bit1 = horizontal.
+ * K3 filters all edges of one direction at once, which is exact only on a legal grid.  Per side, a luma edge of length n
+ * writes n samples and reads 3, 3, 4, 6, 8 for n = 1, 2, 3, 5, 7; on a horizontal edge at a CTU row the P side counts as 3,
+ * and when one side is long (5, 7) the other counts as at least 3.  A grid is legal when no Bs field is 3, no edge with
+ * Bs != 0 lies on the picture's first column (lfV) / row (lfH), an edge with luma Bs != 0 has lengths 1, 2, 3, 5 or 7 and
+ * reads nothing outside the picture, and any two luma edges e1 < e2 of one line (row of lfV, column of lfH) have
+ * e2 - e1 >= writesQ(e1) + readsP(e2) and e2 - e1 >= readsQ(e1) + writesP(e2).  Edges of slices with deblocking disabled
+ * count too.  Returns B200_ERR_PARAM, with the host planes untouched and the reason in b200_last_error(), for an illegal
+ * grid, a chromaFormat other than 0 (4:0:0) or 1 (4:2:0), a bit depth outside 8..12, a width or height that is not a
+ * multiple of 8, a plane stride below its plane's width, dirs & ~3, a ctuSlice entry >= numSlices, numSlices outside
+ * 1..64, a CTU size other than 32 / 64 / 128, or LADF with a number of intervals outside 2..5.
+ * The picture path (b200_picture::lfV / lfH) requires legal grids and does not check them; the grids the reference's
+ * calcFilterStrengths derives, as the glue flattens them, are legal. */
 B200_API int b200_lf_deblock(const b200_geom* g, int16_t* const planes[3], const b200_lf_param* lfV, const b200_lf_param* lfH,
                              const uint8_t* ctuSlice, const b200_lf_slice* slices, int numSlices, const b200_lf_seq* seq, int dirs);
 

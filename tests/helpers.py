@@ -573,3 +573,35 @@ def mc_mismatch(case, a, b, da, db):
         bad = np.argwhere((da != db).any(axis=1))[:, 0]
         return f"{case['name']}: DMVR deltas differ at entries {bad[:5].tolist()}: {da[bad[:5]].tolist()} vs {db[bad[:5]].tolist()}"
     return None
+
+
+# ---- K3: one call shape for every deblocking test (tests/test_k3_*.py)
+def lf_args(case, planes):
+    """The leading arguments of orc_lf_deblock / b200_lf_deblock for a sweep case (synth.lf_sweep) on `planes`: geometry, planes, grids, ctuSlice, slices."""
+    cs = case["ctuSlice"]
+    return (C.byref(case["g"]), abi.plane_ptrs(planes), case["lfV"].ctypes.data, case["lfH"].ctypes.data, None if cs is None else cs.ctypes.data,
+            case["slices"].ctypes.data)
+
+
+def lf_oracle(oracle, case, dirs=3, planes=None):
+    """orc_lf_deblock of a sweep case on copies of its planes (or of `planes`)."""
+    out = [None if p is None else p.copy() for p in (planes or case["planes"])]
+    oracle.orc_lf_deblock(*lf_args(case, out), C.addressof(case["seq"]), dirs)
+    return out
+
+
+def lf_mismatch(oracle, case, got, want, dirs=3):
+    """None when the planes agree (stride padding included); else a message naming the case, the plane, the first differing sample and the decision
+    lf_decisions gives each segment that may write it (with dirs 3, horizontal segments are classified on the oracle's vertical-only output)."""
+    for c, (a, b) in enumerate(zip(got, want)):
+        if b is None or np.array_equal(a, b): continue
+        bad = np.argwhere(a != b); y, x = (int(v) for v in bad[0])
+        seen = []
+        for d in (0, 1):
+            if not dirs & (1 << d): continue
+            start = lf_oracle(oracle, case, 1) if d and dirs & 1 else case["planes"]
+            recs = synth.lf_decisions(start, case["lfH" if d else "lfV"], d, case["g"], case["slices"], case["seq"], case["ctuSlice"])
+            seen += [f"{'H' if d else 'V'} edge ({r['x']}, {r['y']}) {r['tag']}" for r in recs if r["comp"] == c and (y, x) in r["writes"]]
+        return f"{case['name']}: plane {c}: {len(bad)} samples differ, first at (y={y}, x={x}): {a[y, x]} vs {b[y, x]}; written by: {seen or 'no classified segment'}"
+    return None
+

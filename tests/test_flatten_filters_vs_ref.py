@@ -27,6 +27,8 @@ def test_filter_flatteners_round_trip(ref, W, H, ctu):
                                  lfVo.ctypes.data, lfHo.ctypes.data, saoO.ctypes.data, alfO.ctypes.data, *[o.ctypes.data for o in outs], counts)
     assert rc == 0
     assert np.array_equal(lfV.view(np.uint8), lfVo.view(np.uint8)) and np.array_equal(lfH.view(np.uint8), lfHo.view(np.uint8))
+    # the picture path runs these grids unchecked: they must meet the rule b200_lf_deblock enforces
+    assert synth.lf_grid_problems(lfVo, 0, g) == [] and synth.lf_grid_problems(lfHo, 1, g) == []
     assert np.array_equal(alf["ctus"].view(np.uint8), alfO.view(np.uint8))
     assert list(counts) == [alf["lumaCoeff"].shape[0], alf["chromaCoeff"].shape[0], alf["cc"][0].shape[0], alf["cc"][1].shape[0]]
     for k, o in zip(("lumaCoeff", "lumaClip", "chromaCoeff", "chromaClip"), outs): assert np.array_equal(alf[k], o), k
@@ -37,3 +39,19 @@ def test_filter_flatteners_round_trip(ref, W, H, ctu):
         bo = sao["type"][:, c] == 4; eo = sao["type"][:, c] < 4
         assert np.array_equal(sao["band"][bo, c], saoO["band"][bo, c])
         assert np.array_equal(sao["offset"][bo, c, :4], saoO["offset"][bo, c, :4]) and np.array_equal(sao["offset"][eo, c], saoO["offset"][eo, c])
+
+
+@pytest.mark.parametrize("seed,kw", [(1, dict()), (2, dict(ctu=32, bd=8)), (3, dict(ctu=64, slice_type=2, isp=30)), (4, dict(affine=60, split=85)),
+                                     (5, dict(tools=None, slices=3, ctu=32))])
+def test_flattened_deblocking_grids_are_legal(ref, seed, kw):
+    """The grids the glue flattens from the reference's own calcFilterStrengths (sub-block lengths 5 and 2 of affine / SbTMVP CUs, 4-wide CUs, CTU 32
+    rows, intra pictures) meet the rule of the flat pass: the picture path runs them without checking."""
+    from tests import helpers
+    case = helpers.SeamCase(ref, np.random.default_rng(seed), 416, 240, **kw)
+    pic, rc = case.flatten()
+    assert pic is not None, rc
+    W4, H4 = case.W // 4, case.H // 4
+    lfV, lfH = pic["lfV"].reshape(H4, W4), pic["lfH"].reshape(H4, W4)
+    assert synth.lf_grid_problems(lfV, 0, case.g) == [] and synth.lf_grid_problems(lfH, 1, case.g) == []
+    lens = {int(v) >> 4 & 7 for v in lfV["len"][lfV["bs"] & 3 > 0]} | {int(v) & 7 for v in lfV["len"][lfV["bs"] & 3 > 0]}
+    assert lens >= {1, 3}, lens

@@ -80,3 +80,17 @@ def test_deblock_picture_vs_reference(oracle, ref, seed, W, H, bd, ctu, nsl, lad
         assert not np.array_equal(a[c], planes[c]), "deblocking changed nothing — test content too weak"
     # long filters must have been exercised
     assert ((lfV["len"] >> 4) & 7 == 7).any()
+
+
+@pytest.mark.parametrize("simd", [0, 1])
+@pytest.mark.parametrize("name", list(synth.LF_SWEEP_CASES))
+def test_deblock_sweep_vs_reference(oracle, ref, name, simd):
+    """Every case of the designed sweep (synth.lf_sweep) through the real LoopFilter, 4:0:0 and 64 slices included: the oracle's planes equal the
+    reference's, stride padding included."""
+    from tests.helpers import lf_args, lf_oracle, lf_mismatch
+    case = synth.lf_sweep(name)
+    want = lf_oracle(oracle, case)
+    got = [None if p is None else p.copy() for p in case["planes"]]
+    ref.ref_lf_deblock_picture(simd, *lf_args(case, got), len(case["slices"]), C.addressof(case["seq"]), 3)
+    msg = lf_mismatch(oracle, case, got, want)
+    assert msg is None, msg

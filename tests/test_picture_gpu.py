@@ -396,3 +396,42 @@ def test_work_lists_and_dmvr_deltas_in_arrays_that_start_in_a_registered_page(b2
     finally:
         if ctx: b200.b200_ctx_destroy(ctx)
         b200.b200_host_unregister(raw.ctypes.data + base); b200.b200_host_unregister(rawp.ctypes.data + basep)
+
+
+@pytest.mark.parametrize("name,strides", [("tight_spacing", None), ("ctu_edges_ctu32_200x136", (201, 103, 100)), ("qp_ladf_10bit", None)])
+def test_designed_deblocking_in_a_picture(b200, oracle, name, strides):
+    """Cases of the designed K3 sweep (synth.lf_sweep) through b200_decompress_picture: the designed planes as `given`, no PUs or TUs, deblocking on with
+    the case's grids, slices and LADF; the CTU-32 case with an odd luma stride.  The frame equals the oracle chain's."""
+    case = synth.lf_sweep(name)
+    W, H, bd, ctu = case["W"], case["H"], case["bd"], case["ctu"]
+    g = abi.make_geom(W, H, bd, ctu=ctu, strides=strides)
+    given = []
+    for c in range(3):
+        w, h = (W, H) if c == 0 else (W // 2, H // 2)
+        p = np.zeros((h, g.stride[c]), np.int16); p[:, :w] = case["planes"][c][:, :w]; given.append(p)
+    pic = synth.gen_picture(np.random.default_rng(3), W, H, bd, ctu=ctu, dst_slot=4, inter=False, tu_kw=dict(p_cbf=0.0), deblock=False, sao=False, alf=False)
+    st = pic["struct"]
+    assert len(pic["pus"]) == 0 and len(pic["tus"]) == 0
+    pic["given"] = given
+    for c in range(3): st.given[c] = given[c].ctypes.data
+    pic["lfV"], pic["lfH"], pic["lfSlices"], pic["lfSeq"] = case["lfV"], case["lfH"], case["slices"], case["seq"]
+    st.flags |= abi.PIC_DEBLOCK; st.lfV = case["lfV"].ctypes.data; st.lfH = case["lfH"].ctypes.data
+    st.lfSlices = case["slices"].ctypes.data; st.numLfSlices = len(case["slices"]); st.lfSeq = C.addressof(case["seq"])
+    if case["ctuSlice"] is not None: pic["ctuSlice"] = case["ctuSlice"]; st.ctuSlice = case["ctuSlice"].ctypes.data
+    refs = [[np.zeros_like(p) for p in given] for _ in range(4)]
+    want, _ = oracle_decompress(oracle, g, refs, pic)
+    assert not np.array_equal(want[0], given[0])
+    ctx = C.c_void_p()
+    vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 2, -1))
+    try:
+        h = b200.b200_decompress_picture(ctx, C.byref(st))
+        assert h >= 0, b200.b200_last_error()
+        vvdec_b200.check(b200.b200_wait_picture(ctx, h, None, 0))
+        got = [np.zeros_like(p) for p in given]
+        vvdec_b200.check(b200.b200_get_frame(ctx, 4, abi.plane_ptrs(got)))
+        for c in range(3):
+            w, hh = (W, H) if c == 0 else (W // 2, H // 2)
+            bad = np.argwhere(want[c][:hh, :w] != got[c][:hh, :w])
+            assert len(bad) == 0, f"{name}: plane {c}: {len(bad)} diffs, first at {bad[:1].tolist()}"
+    finally:
+        b200.b200_ctx_destroy(ctx)

@@ -123,12 +123,59 @@ B200_API int b200_k1_residual(const b200_geom* g, int16_t* const planes[3], cons
   return 0;
 }
 
+// Samples a luma edge side of effective length n reads: n + 1 (its filters' reference sample), and p2/q2 for the decisions of lengths 1 and 2.
+static int lf_reads(int n) { return n < 3 ? 3 : n + 1; }
+
+// K3's flat pass (k3_deblock.cu) is exact only when no edge reads a sample that another edge of the same direction writes, and it reads no sample
+// outside the plane.  One raster scan of a grid; returns false with the error set at the first edge that breaks a rule (include/vvdec_b200.h).
+static bool lf_grid_legal(const b200_geom& g, const b200_lf_param* grid, int dir)
+{
+  const int W4 = g.width >> 2, H4 = g.height >> 2, extent = dir ? g.height : g.width;
+  const char* name = dir ? "lfH" : "lfV";
+  std::vector<int> prev(dir ? W4 : H4, -1), prevWQ(prev.size()), prevRQ(prev.size());   // per line: the last luma edge and its Q side's writes / reads
+  for (int y4 = 0; y4 < H4; y4++)
+    for (int x4 = 0; x4 < W4; x4++) {
+      const b200_lf_param& e = grid[(size_t)y4 * W4 + x4];
+      const int bs = e.bs & 0x3f, line = dir ? x4 : y4, pos = 4 * (dir ? y4 : x4);
+      if (!bs) continue;
+      if ((bs & 3) == 3 || ((bs >> 2) & 3) == 3 || (bs >> 4) == 3) { set_error("b200_lf_deblock: %s edge at (%d, %d): Bs 3", name, 4 * x4, 4 * y4); return false; }
+      if (pos == 0) { set_error("b200_lf_deblock: %s edge at (%d, %d): Bs != 0 on the picture's border", name, 4 * x4, 4 * y4); return false; }
+      if (!(bs & 3)) continue;                                  // chroma only: 4:2:0 chroma edges are 8 samples apart and read 4 per side
+      int nP = (e.sideMaxFiltLength >> 4) & 7;
+      const int nQ = e.sideMaxFiltLength & 7;
+      const auto ok = [](int n) { return n == 1 || n == 2 || n == 3 || n == 5 || n == 7; };
+      if (!ok(nP) || !ok(nQ)) { set_error("b200_lf_deblock: %s edge at (%d, %d): luma filter lengths %d/%d (1, 2, 3, 5 or 7)", name, 4 * x4, 4 * y4, nP, nQ); return false; }
+      if (dir && (pos & (g.ctuSize - 1)) == 0 && nP > 3) nP = 3;   // a CTU row: the P side is never large
+      const bool large = nP > 3 || nQ > 3;                       // the long filter runs a short side as length 3
+      const int wP = large ? std::max(nP, 3) : nP, wQ = large ? std::max(nQ, 3) : nQ, rP = lf_reads(wP), rQ = lf_reads(wQ);
+      if (pos < rP || pos + rQ > extent) { set_error("b200_lf_deblock: %s edge at (%d, %d): lengths %d/%d read outside the picture", name, 4 * x4, 4 * y4, nP, nQ); return false; }
+      if (prev[line] >= 0 && (pos - prev[line] < prevWQ[line] + rP || pos - prev[line] < prevRQ[line] + wP)) {
+        set_error("b200_lf_deblock: %s edge at (%d, %d): reads or writes samples the edge %d samples before it writes or reads", name, 4 * x4, 4 * y4, pos - prev[line]);
+        return false;
+      }
+      prev[line] = pos; prevWQ[line] = wQ; prevRQ[line] = rQ;
+    }
+  return true;
+}
+
 B200_API int b200_lf_deblock(const b200_geom* g, int16_t* const planes[3], const b200_lf_param* lfV, const b200_lf_param* lfH,
                              const uint8_t* ctuSlice, const b200_lf_slice* slices, int numSlices, const b200_lf_seq* seq, int dirs)
 {
   B200_CHECK(g && planes && lfV && lfH && slices, "b200_lf_deblock: null argument");
   B200_CHECK(numSlices >= 1 && numSlices <= 64, "b200_lf_deblock: numSlices %d out of range 1..64", numSlices);
   B200_CHECK(g->ctuSize == 32 || g->ctuSize == 64 || g->ctuSize == 128, "b200_lf_deblock: CTU size %d", g->ctuSize);
+  // K3 filters 4:0:0 and 4:2:0 only; any other format would upload three planes and leave chroma unfiltered
+  B200_CHECK(g->chromaFormat == 0 || g->chromaFormat == 1, "b200_lf_deblock: chromaFormat %d (only 0 = 4:0:0 and 1 = 4:2:0)", g->chromaFormat);
+  B200_CHECK(g->bitDepth >= 8 && g->bitDepth <= 12, "b200_lf_deblock: bit depth %d (8..12)", g->bitDepth);
+  B200_CHECK(g->width > 0 && g->height > 0 && !(g->width & 7) && !(g->height & 7), "b200_lf_deblock: picture %dx%d is not a multiple of 8", g->width, g->height);
+  B200_CHECK(g->stride[0] >= g->width && (!g->chromaFormat || (g->stride[1] >= g->width / 2 && g->stride[2] >= g->width / 2)),
+             "b200_lf_deblock: a plane stride is smaller than the plane's width");
+  B200_CHECK(!(dirs & ~3), "b200_lf_deblock: dirs %d (bit 0 vertical, bit 1 horizontal edges)", dirs);
+  B200_CHECK(!seq || !seq->ladfEnabled || (seq->ladfNumIntervals >= 2 && seq->ladfNumIntervals <= 5), "b200_lf_deblock: %d LADF intervals (2..5)", seq ? seq->ladfNumIntervals : 0);
+  const size_t n4 = (size_t)((g->width + 3) >> 2) * ((g->height + 3) >> 2);
+  const size_t nCtu = (size_t)((g->width + g->ctuSize - 1) / g->ctuSize) * ((g->height + g->ctuSize - 1) / g->ctuSize);
+  for (size_t i = 0; ctuSlice && i < nCtu; i++) B200_CHECK(ctuSlice[i] < numSlices, "b200_lf_deblock: CTU %zu is in slice %d of %d", i, ctuSlice[i], numSlices);
+  if (!lf_grid_legal(*g, lfV, 0) || !lf_grid_legal(*g, lfH, 1)) return B200_ERR_PARAM;
   if (int rc = ensure_device()) return rc;
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
@@ -136,8 +183,6 @@ B200_API int b200_lf_deblock(const b200_geom* g, int16_t* const planes[3], const
   memset(&L.slices, 0, sizeof(L.slices)); memcpy(L.slices.s, slices, numSlices * sizeof(b200_lf_slice));
   if (seq) L.seq = *seq; else memset(&L.seq, 0, sizeof(L.seq));
   if (int rc = upload_planes(g, planes, L.planes, s)) return rc;
-  const size_t n4 = (size_t)((g->width + 3) >> 2) * ((g->height + 3) >> 2);
-  const size_t nCtu = (size_t)((g->width + g->ctuSize - 1) / g->ctuSize) * ((g->height + g->ctuSize - 1) / g->ctuSize);
   if (int rc = g_hw.misc[0].reserve(n4 * sizeof(b200_lf_param))) return rc;
   if (int rc = g_hw.misc[1].reserve(n4 * sizeof(b200_lf_param))) return rc;
   if (int rc = g_hw.misc[2].reserve(nCtu)) return rc;

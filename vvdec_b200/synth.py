@@ -1305,3 +1305,514 @@ def mc_sweep(name):
                 tags=tags, marks=marks, targets=targets, wp=wp)
     _mc_sweep_cache[name] = case
     return case
+
+
+# ---- K3: decisions, the grid rule of the flat pass and the designed deblocking sweep (tests/test_k3_*.py)
+LF_TC = (0,) * 18 + (3, 4, 4, 4, 4, 5, 5, 5, 5, 7, 7, 8, 9, 10, 10, 11, 13, 14, 15, 17, 19, 21, 24, 25, 29, 33, 36, 41, 45, 51, 57, 64, 71, 80, 89, 100, 112,
+                     125, 141, 157, 177, 198, 222, 250, 280, 314, 352, 395)              # H.266 Table 43, tC'
+LF_BETA = (0,) * 16 + tuple(range(6, 19)) + tuple(range(20, 89, 2))                      # H.266 Table 43, beta'
+assert len(LF_TC) == 66 and len(LF_BETA) == 64
+
+
+def lf_tc(idx, bd):
+    return (LF_TC[idx] + (1 << (9 - bd))) >> (10 - bd) if bd < 10 else LF_TC[idx] << (bd - 10)
+
+
+def lf_beta(idx, bd):
+    return LF_BETA[idx] << (bd - 8)
+
+
+def _clip(lo, hi, v):
+    return lo if v < lo else hi if v > hi else v
+
+
+def _lf_line(plane, x, y, d, line, n):
+    """The samples across an edge on one line, counted from the edge: (p[0..n-1], q[0..n-1]); samples outside the array read as 0."""
+    h, w = plane.shape
+    at = lambda r, c: int(plane[r, c]) if 0 <= r < h and 0 <= c < w else 0
+    if d == 0: return [at(y + line, x - 1 - k) for k in range(n)], [at(y + line, x + k) for k in range(n)]
+    return [at(y - 1 - k, x + line) for k in range(n)], [at(y + k, x + line) for k in range(n)]
+
+
+def _lf_at(x, y, d, line, side, k):
+    """(row, column) of the k-th sample of the P (side 0) or Q (side 1) side of one line."""
+    o = -1 - k if side == 0 else k
+    return (y + line, x + o) if d == 0 else (y + o, x + line)
+
+
+def _lf_strong(p, q, d, beta, tc, largeP, largeQ, maxP, maxQ, ctb=False):
+    """xUseStrongFiltering (LoopFilter.cpp:1410) on one line: (decision, sp3 + sq3 as compared)."""
+    ok = d < (beta >> 2) and abs(p[0] - q[0]) < ((tc * 5 + 1) >> 1)
+    sp, sq = abs(p[1] - p[0]) if ctb else abs(p[3] - p[0]), abs(q[3] - q[0])
+    if largeP or largeQ:
+        if largeP:
+            if maxP == 7: sp += abs(p[4] - p[5] - p[6] + p[7])
+            sp = (sp + abs(p[3] - p[maxP]) + 1) >> 1
+        if largeQ:
+            if maxQ == 7: sq += abs(q[4] - q[5] - q[6] + q[7])
+            sq = (sq + abs(q[maxQ] - q[3]) + 1) >> 1
+        return ok and sp + sq < (beta * 3 >> 5) and d < (beta >> 4), sp + sq
+    return ok and sp + sq < (beta >> 3), sp + sq
+
+
+def _lf_luma(P, x, y, d, e, sl, seq, bd, ctu):
+    """xEdgeFilterLuma's decisions (LoopFilter.cpp:1463) for one 4-line segment."""
+    bs, qp, pmax = int(e["bs"]) & 3, int(e["qp"][0]), (1 << bd) - 1
+    if seq is not None and seq.ladfEnabled:                    # deriveLADFShift :1363
+        (p0, q0), (p3, q3) = _lf_line(P, x, y, d, 0, 1), _lf_line(P, x, y, d, 3, 1)
+        lvl, shift = (q0[0] + q3[0] + p0[0] + p3[0]) >> 2, seq.ladfQpOffset[0]
+        for k in range(1, seq.ladfNumIntervals):
+            if lvl > seq.ladfIntervalLowerBound[k]: shift = seq.ladfQpOffset[k]
+            else: break
+        qp += shift
+    maxP, maxQ = (int(e["len"]) >> 4) & 7, int(e["len"]) & 7
+    largeP, largeQ = maxP > 3 and not (d == 1 and y % ctu == 0), maxQ > 3
+    itc, ib = _clip(0, 65, qp + 2 * (bs - 1) + 2 * int(sl["tc"][0])), _clip(0, 63, qp + 2 * int(sl["beta"][0]))
+    tc, beta = lf_tc(itc, bd), lf_beta(ib, bd)
+    L = [_lf_line(P, x, y, d, l, 8) for l in range(4)]
+    dp = [abs(p[2] - 2 * p[1] + p[0]) for p, q in L]; dq = [abs(q[0] - 2 * q[1] + q[2]) for p, q in L]
+    Q = dict(qp=qp, itc=itc, ib=ib, tc=tc, beta=beta, beta2=beta >> 2, beta3=beta >> 3, beta4=beta >> 4, beta35=beta * 3 >> 5, tc25=(tc * 5 + 1) >> 1,
+             sideThr=(beta + (beta >> 1)) >> 3, thrCut=tc * 10, dsum=dp[0] + dq[0] + dp[3] + dq[3], pq_a=abs(L[0][0][0] - L[0][1][0]), pq_b=abs(L[3][0][0] - L[3][1][0]))
+    side = lambda n, m: {(l, 0, k) for l in range(4) for k in range(n)} | {(l, 1, k) for l in range(4) for k in range(m)}
+    if largeP or largeQ:
+        dL = [(((dp[l] + abs(L[l][0][5] - 2 * L[l][0][4] + L[l][0][3]) + 1) >> 1) if largeP else dp[l]) +
+              (((dq[l] + abs(L[l][1][3] - 2 * L[l][1][4] + L[l][1][5]) + 1) >> 1) if largeQ else dq[l]) for l in (0, 3)]
+        sa, sb = (_lf_strong(*L[l], 2 * dL[i], beta, tc, largeP, largeQ, maxP, maxQ) for i, l in enumerate((0, 3)))
+        Q.update(dsumL=dL[0] + dL[1], d2L_a=2 * dL[0], d2L_b=2 * dL[1], sL_a=sa[1], sL_b=sb[1])
+        if Q["dsumL"] < beta and sa[0] and sb[0]:
+            nP, nQ = maxP if largeP else 3, maxQ if largeQ else 3
+            return f"long{nP}{nQ}", side(nP, nQ), Q
+    if Q["dsum"] >= beta: return "none", set(), Q
+    fP = fQ = sw = False
+    if maxP > 1 and maxQ > 1: fP, fQ = dp[0] + dp[3] < Q["sideThr"], dq[0] + dq[3] < Q["sideThr"]
+    Q.update(pside=dp[0] + dp[3], qside=dq[0] + dq[3])
+    if maxP > 2 and maxQ > 2:
+        sa, sb = (_lf_strong(*L[l], 2 * (dp[l] + dq[l]), beta, tc, False, False, 7, 7) for l in (0, 3))
+        Q.update(d2_a=2 * (dp[0] + dq[0]), d2_b=2 * (dp[3] + dq[3]), s_a=sa[1], s_b=sb[1])
+        sw = sa[0] and sb[0]
+    if sw: return "strong", side(3, 3), Q
+    writes, deltas, clip01 = set(), [], False
+    for l, (p, q) in enumerate(L):
+        delta = (9 * (q[0] - p[0]) - 3 * (q[1] - p[1]) + 8) >> 4
+        deltas.append(delta)
+        if abs(delta) >= Q["thrCut"]: continue
+        dc, t2 = _clip(-tc, tc, delta), tc >> 1
+        new = [p[0] + dc, q[0] - dc] + ([p[1] + _clip(-t2, t2, (((p[2] + p[0] + 1) >> 1) - p[1] + dc) >> 1)] if fP else []) + \
+              ([q[1] + _clip(-t2, t2, (((q[2] + q[0] + 1) >> 1) - q[1] - dc) >> 1)] if fQ else [])
+        clip01 |= any(v < 0 or v > pmax for v in new)
+        writes |= {(l, 0, 0), (l, 1, 0)} | ({(l, 0, 1)} if fP else set()) | ({(l, 1, 1)} if fQ else set())
+    Q.update(adelta_a=abs(deltas[0]), adelta_b=abs(deltas[3]), clip01=clip01)
+    return ("weak_cut" if not writes else f"weak{int(fP)}{int(fQ)}"), writes, Q
+
+
+def _lf_chroma(P, cx, cy, d, e, sl, c, bd, ctu):
+    """xEdgeFilterChroma's decisions (LoopFilter.cpp:1619) for one 2-line segment of component c (4:2:0)."""
+    bs, large = (int(e["bs"]) >> (2 * c)) & 3, (int(e["flags"]) >> 5) & 1
+    ctb = d == 1 and cy % (ctu >> 1) == 0
+    sfx = "_ctb" if ctb else ""
+    if not (bs == 2 or (large and bs == 1)): return "none" + sfx, set(), {}
+    qp = int(e["qp"][c])
+    itc = _clip(0, 65, qp + 2 * (bs - 1) + 2 * int(sl["tc"][c])); tc = lf_tc(itc, bd)
+    Q = dict(qp=qp, itc=itc, tc=tc, tc25=(tc * 5 + 1) >> 1)
+    weak = {(l, s, 0) for l in range(2) for s in range(2)}
+    if not large: return "chroma_weak_small" + sfx, weak, Q
+    ib = _clip(0, 63, qp + 2 * int(sl["beta"][c])); beta = lf_beta(ib, bd)
+    L = [_lf_line(P, cx, cy, d, l, 4) for l in range(2)]
+    dl = [(abs(p[0] - p[1]) if ctb else abs(p[2] - 2 * p[1] + p[0])) + abs(q[0] - 2 * q[1] + q[2]) for p, q in L]
+    Q.update(ib=ib, beta=beta, beta2=beta >> 2, beta3=beta >> 3, dsum=dl[0] + dl[1], d2_a=2 * dl[0], d2_b=2 * dl[1],
+             pq_a=abs(L[0][0][0] - L[0][1][0]), pq_b=abs(L[1][0][0] - L[1][1][0]))
+    if Q["dsum"] >= beta: return "chroma_weak_d" + sfx, weak, Q
+    sa, sb = (_lf_strong(*L[l], 2 * dl[l], beta, tc, False, False, 7, 7, ctb) for l in range(2))
+    Q.update(s_a=sa[1], s_b=sb[1])
+    if sa[0] and sb[0]:
+        return "chroma_strong" + sfx, {(l, 0, k) for l in range(2) for k in range(1 if ctb else 3)} | {(l, 1, k) for l in range(2) for k in range(3)}, Q
+    return "chroma_weak" + sfx, weak, Q
+
+
+def lf_decisions(planes, grid, d, g, slices, seq=None, ctu_slice=None):
+    """The decisions of xEdgeFilterLuma / xEdgeFilterChroma (not the filters) for every segment of one direction's grid (d: 0 lfV, 1 lfH) on `planes`,
+    the picture that direction starts from (for lfH: the output of the vertical pass).  Returns one dict per segment: dir, comp, x / y (the first Q
+    sample, in the component's plane), tag (none, weak00..weak11, weak_cut, strong, long<P><Q>, chroma_weak_small / _d / chroma_weak / chroma_strong,
+    + _ctb at a chroma CTB row, off in a slice with deblocking disabled), writes (the (row, column) samples the decision may change) and q (the
+    quantities and thresholds it compared)."""
+    out = []
+    bd, ctu = g.bitDepth, g.ctuSize
+    ctus_w = (g.width + ctu - 1) // ctu
+    ys, xs = np.nonzero(grid["bs"] & 0x3f)
+    for y4, x4 in zip(ys.tolist(), xs.tolist()):
+        e, x, y = grid[y4, x4], 4 * x4, 4 * y4
+        sl = slices[int(ctu_slice[(y // ctu) * ctus_w + x // ctu]) if ctu_slice is not None else 0]
+        segs = []
+        if int(e["bs"]) & 3: segs.append((0, x, y, 4))
+        if g.chromaFormat == 1 and int(e["bs"]) >> 2 and (x if d == 0 else y) % 16 == 0:
+            segs += [(c, x >> 1, y >> 1, 2) for c in (1, 2) if (int(e["bs"]) >> (2 * c)) & 3]
+        for c, cx, cy, n in segs:
+            if sl["disable"]: tag, w, q = "off", set(), {}
+            elif c == 0: tag, w, q = _lf_luma(planes[0], x, y, d, e, sl, seq, bd, ctu)
+            else: tag, w, q = _lf_chroma(planes[c], cx, cy, d, e, sl, c, bd, ctu)
+            out.append(dict(dir=d, comp=c, x=cx, y=cy, tag=tag, q=q, writes={_lf_at(cx, cy, d, l, s, k) for l, s, k in w}))
+    return out
+
+
+LF_READS = {1: 3, 2: 3, 3: 4, 5: 6, 7: 8}
+
+
+def lf_grid_problems(grid, d, g, limit=8):
+    """What the flat pass of K3 needs from one direction's grid (d: 0 lfV, 1 lfH), as b200_lf_deblock checks it: the first `limit` edges that break a
+    rule, as strings (empty: legal).  Per side, a luma edge of length n writes n samples and reads LF_READS[n]; on a horizontal edge at a CTU row the P
+    side counts as 3, and when one side is long (5, 7) the other counts as at least 3 (the long filter runs it as 3).  Rules: Bs fields are 0..2; no
+    edge with Bs != 0 on the picture's first column (lfV) / row (lfH); luma lengths of an edge with luma Bs != 0 are 1, 2, 3, 5 or 7; no side reads past
+    the picture; and two luma edges at e1 < e2 on one line need e2 - e1 >= writesQ(e1) + readsP(e2) and e2 - e1 >= readsQ(e1) + writesP(e2)."""
+    out = []
+    bs = grid["bs"].astype(np.int64) & 0x3f
+    extent = g.height if d else g.width
+    lines, poss = np.nonzero(bs.T if d else bs)
+    prev = {}
+    for line, k in zip(lines.tolist(), poss.tolist()):
+        y4, x4 = (k, line) if d else (line, k)
+        e, pos, where = grid[y4, x4], 4 * k, f"{'lfH' if d else 'lfV'} ({4 * x4}, {4 * y4})"
+        b = int(e["bs"]) & 0x3f
+        if 3 in (b & 3, (b >> 2) & 3, b >> 4): out.append(f"{where}: Bs 3")
+        elif pos == 0: out.append(f"{where}: Bs != 0 on the picture's border")
+        elif b & 3:
+            nP, nQ = (int(e["len"]) >> 4) & 7, int(e["len"]) & 7
+            if nP not in LF_READS or nQ not in LF_READS: out.append(f"{where}: luma lengths {nP}/{nQ}"); continue
+            if d and pos % g.ctuSize == 0: nP = min(nP, 3)
+            wP, wQ = (max(nP, 3), max(nQ, 3)) if max(nP, nQ) > 3 else (nP, nQ)
+            rP, rQ = LF_READS[wP], LF_READS[wQ]
+            if pos < rP or pos + rQ > extent: out.append(f"{where}: lengths {nP}/{nQ} read outside the picture")
+            elif line in prev and (pos - prev[line][0] < prev[line][1] + rP or pos - prev[line][0] < prev[line][2] + wP):
+                out.append(f"{where}: {pos - prev[line][0]} samples after the previous edge")
+            prev[line] = (pos, wQ, rQ)
+        if len(out) >= limit: break
+    return out
+
+
+def lf_grid_legal(grid, d, g):
+    return not lf_grid_problems(grid, d, g, limit=1)
+
+
+def _lf_side(v, d=0, s=0, dx=0, e=0, a1=0):
+    """Eight samples of one side of an edge, nearest first, around level v: |x2 - 2 x1 + x0| = d, |x3 - x0| = s, |x5 - 2 x4 + x3| = dx, and at length 7
+    |x4 - x5 - x6 + x7| = e with x7 = x3 (length 5: |x3 - x5| = dx); a1 = x1 - x0 (the chroma CTB form's |p1 - p0|)."""
+    return [v, v + a1, v + d + 2 * a1, v + s, v + s, v + s + dx, v + s - dx - e, v + s]
+
+
+class _LfCanvas:
+    """A picture being laid out for the deblocking sweep: planes at mid grey, empty grids, and the designed segments placed so far."""
+    def __init__(self, W, H, bd, ctu, chroma=1, strides=None, fill=-7):
+        self.g = abi.make_geom(W, H, bd, chroma_format=chroma, ctu=ctu, strides=strides or ((W, W >> 1, W >> 1) if chroma else (W, 0, 0)))
+        self.W, self.H, self.bd, self.ctu, self.chroma = W, H, bd, ctu, chroma
+        mid = 1 << (bd - 1)
+        self.planes = [None, None, None]
+        for c in range(3 if chroma else 1):
+            w, h = (W, H) if c == 0 else (W >> 1, H >> 1)
+            self.planes[c] = np.full((h, self.g.stride[c]), fill, np.int16); self.planes[c][:, :w] = mid
+        self.lf = [np.zeros((H // 4, W // 4), LF_DTYPE) for _ in range(2)]
+        self.segs = []
+
+    def put(self, spec, d, x, y):
+        """Writes a designed segment across the edge at luma (x, y): spec = dict(tag, comp (0 luma, 'c' both chroma), lens, bs, qp, large, lines,
+        probes) where lines are the (p, q) sample lists of each line (4 luma, 2 chroma)."""
+        e = self.lf[d][y // 4, x // 4]
+        comps = (0,) if spec.get("comp", 0) == 0 else (1, 2)
+        bs = spec.get("bs", 2)
+        e["bs"] = bs if comps == (0,) else (bs << 2) | (bs << 4)
+        e["len"] = 128 + (spec.get("lens", (3, 3))[0] << 4) + spec.get("lens", (3, 3))[1]
+        e["flags"] = 32 if spec.get("large") else 0
+        e["qp"] = (spec.get("qp", 37),) * 3
+        for c in comps:
+            cx, cy = (x, y) if c == 0 else (x >> 1, y >> 1)
+            for l, (p, q) in enumerate(spec["lines"]):
+                for s, vals in ((0, p), (1, q)):
+                    for k, v in enumerate(vals[:8 if c == 0 else 4]): self.planes[c][_lf_at(cx, cy, d, l, s, k)] = v    # a chroma slot holds 4 per side
+            self.segs.append(dict(dir=d, comp=c, x=cx, y=cy, tag=spec["tag"], probes=spec.get("probes", [])))
+
+    def case(self, name, slices=None, ctu_slice=None, seq=None, classify=True):
+        return dict(name=name, g=self.g, W=self.W, H=self.H, bd=self.bd, ctu=self.ctu, chroma=self.chroma, strides=tuple(self.g.stride),
+                    planes=self.planes, lfV=np.ascontiguousarray(self.lf[0]), lfH=np.ascontiguousarray(self.lf[1]),
+                    slices=np.zeros(1, LFSLICE_DTYPE) if slices is None else slices, ctuSlice=ctu_slice, seq=seq or abi.LfSeq(), segs=self.segs, classify=classify)
+
+
+def _lf_spec(tag, l0, l3=None, v=512, lens=(3, 3), bs=2, qp=37, probes=(), nlines=4, **kw):
+    """A designed segment: line 0 (and the lines up to the last) shaped by l0 = dict(t, dp, dq, sp, sq, dpx, dqx, ep, eq, ap, aq) around level v (Q side at
+    v + t); the last line (3 luma, 1 chroma) by l0 updated with l3."""
+    def line(k):
+        t = k.get("t", 20)
+        return (_lf_side(v, k.get("dp", 0), k.get("sp", 0), k.get("dpx", 0), k.get("ep", 0), k.get("ap", 0)),
+                _lf_side(v + t, k.get("dq", 0), k.get("sq", 0), k.get("dqx", 0), k.get("eq", 0), k.get("aq", 0)))
+    last = dict(l0, **(l3 or {}))
+    return dict(tag=tag, lens=lens, bs=bs, qp=qp, probes=list(probes), lines=[line(l0)] * (nlines - 1) + [line(last)], **kw)
+
+
+def lf_luma_specs():
+    """The designed luma segments (10 bit): thresholds of every decision of xEdgeFilterLuma on both sides.  qp 37 / Bs 2: beta 144, tc 21 (beta>>2 36,
+    beta>>3 18, side threshold 27, (5 tc + 1)>>1 53); qp 39: beta 160, tc 25 (beta>>4 10, 3 beta>>5 15, 63); qp 18 / Bs 1: beta 32, tc 3 (thrCut 30)."""
+    S = []
+    # no filter at d0 + d3 == beta, weak below
+    S += [_lf_spec("none", dict(dp=5, dq=66), dict(dq=68), probes=[("dsum", "beta", 0)]),
+          _lf_spec("weak10", dict(dp=5, dq=66), dict(dq=67), probes=[("dsum", "beta", -1)])]
+    # |delta| at thrCut and one below (flat sides: delta = (6 t + 8) >> 4)
+    S += [_lf_spec("weak_cut", dict(t=79), qp=18, bs=1, probes=[("adelta_a", "thrCut", 0)]),
+          _lf_spec("weak11", dict(t=76), qp=18, bs=1, probes=[("adelta_a", "thrCut", -1)])]
+    # the side taps at the side threshold and one below (sp3 20 keeps strong off)
+    for fP in (0, 1):
+        for fQ in (0, 1):
+            S.append(_lf_spec(f"weak{fP}{fQ}", dict(t=30, sp=20, dp=13, dq=13), dict(dp=14 - fP, dq=14 - fQ),
+                              probes=[("pside", "sideThr", -fP), ("qside", "sideThr", -fQ)]))
+    # delta clipped to +-tc (and exactly tc)
+    S += [_lf_spec("weak11", dict(t=60), probes=[("adelta_a", "tc", 2)]), _lf_spec("weak11", dict(t=-60), v=600, probes=[("adelta_a", "tc", 1)]),
+          _lf_spec("weak11", dict(t=56), probes=[("adelta_a", "tc", 0)]), _lf_spec("weak11", dict(t=53), probes=[("adelta_a", "tc", -1)])]
+    # normal strong, and each of its conditions failing alone on line 0 only and on line 3 only
+    base = dict(dp=2, dq=2, t=20)
+    S.append(_lf_spec("strong", base, probes=[("d2_a", "beta2", -28), ("pq_a", "tc25", -33), ("s_a", "beta3", -18)]))
+    for ln, key in ((0, "a"), (3, "b")):
+        for cond, fail, ok, q, thr, okoff in (("d", dict(dp=9, dq=9), dict(dp=8, dq=9), "d2", "beta2", -2), ("pq", dict(t=53), dict(t=52), "pq", "tc25", -1),
+                                              ("s", dict(sp=18), dict(sp=17), "s", "beta3", -1)):
+            for tag, ch, off in (("weak11", fail, 0), ("strong", ok, okoff)):
+                l0, l3 = (dict(base, **ch), dict(base)) if ln == 0 else (base, ch)
+                S.append(_lf_spec(tag, l0, l3, probes=[(f"{q}_{key}", thr, off)]))
+    # every long pair, and each long condition failing alone on line 0 (the segment then takes the normal decision)
+    for P, Q in ((5, 3), (3, 5), (5, 5), (5, 7), (7, 5), (7, 3), (3, 7), (7, 7)):
+        big = "p" if P > 3 else "q"
+        S.append(_lf_spec(f"long{P}{Q}", dict(t=20), lens=(P, Q), qp=39, probes=[("d2L_a", "beta4", -10), ("sL_a", "beta35", -15), ("pq_a", "tc25", -43)]))
+        for fail, ok, q, thr, off, ftag in ((dict(**{f"d{big}x": 9}), dict(**{f"d{big}x": 7}), "d2L_a", "beta4", -2, "strong"),
+                                            (dict(**{f"s{big}": 29}), dict(**{f"s{big}": 27}), "sL_a", "beta35", -1, "weak11"),
+                                            (dict(t=63), dict(t=62), "pq_a", "tc25", -1, "weak11")):
+            S.append(_lf_spec(ftag, dict({"t": 20}, **fail), dict(t=20), lens=(P, Q), qp=39, probes=[(q, thr, 0)]))
+            S.append(_lf_spec(f"long{P}{Q}", dict({"t": 20}, **ok), dict(t=20), lens=(P, Q), qp=39, probes=[(q, thr, off)]))
+    # lengths 1/1 and 2/2: strong is off on content that would take it, the side taps follow the length
+    S += [_lf_spec("weak00", base, lens=(1, 1)), _lf_spec("weak11", base, lens=(2, 2)), _lf_spec("weak01", dict(base, dp=13), dict(dp=14), lens=(2, 2))]
+    return S
+
+
+def lf_chroma_specs(ctb):
+    """The designed chroma segments (10 bit, qp 37: beta 144, tc 21 at Bs 2 / 17 at Bs 1): Bs 1 / 2 x large 0 / 1, and a large edge's strong filter
+    failing one condition at a time; ctb: the forms of a horizontal CTB boundary (P side of two rows)."""
+    sfx, C = ("_ctb" if ctb else ""), []
+    sp = lambda k: dict(ap=k) if ctb else dict(sp=k)          # what sp3 measures: |p1 - p0| at a CTB boundary, else |p3 - p0|
+    spec = lambda tag, l0, l1=None, **kw: _lf_spec(tag + sfx, l0, l1, nlines=2, comp="c", **kw)
+    C += [spec("none", dict(t=20), bs=1), spec("chroma_weak_small", dict(t=20)), spec("chroma_strong", dict(t=20), bs=1, large=1),
+          spec("chroma_strong", dict(t=20), large=1, probes=[("pq_a", "tc25", -33)]),
+          spec("chroma_weak_d", dict(dq=72), large=1, probes=[("dsum", "beta", 0)]), spec("chroma_weak", dict(dq=72), dict(dq=71), large=1, probes=[("dsum", "beta", -1)])]
+    for ln, key in ((0, "a"), (1, "b")):
+        for fail, ok, q, thr, off in ((dict(dq=18), dict(dq=17), "d2", "beta2", -2), (dict(t=53), dict(t=52), "pq", "tc25", -1), (dict(sq=18), dict(sq=17), "s", "beta3", -1)):
+            for tag, ch, o in (("chroma_weak", fail, 0), ("chroma_strong", ok, off)):
+                l0, l1 = (dict({"t": 20}, **ch), dict(t=20)) if ln == 0 else (dict(t=20), dict({"t": 20}, **ch))
+                C.append(spec(tag, l0, l1, large=1, probes=[(f"{q}_{key}", thr, o)]))
+    C.append(spec("chroma_weak", dict({"t": 20}, **sp(18)), large=1, probes=[("s_a", "beta3", 0)]))
+    return C
+
+
+def _lf_layout(cv, vspecs, hspecs, y0=0):
+    """Places segments: vertical edges in 32 x 4 luma slots from row y0 (edge at +16), horizontal ones in 4 x 16 slots below (edge at +8, on the 16-row
+    chroma grid); a horizontal spec with ctb=True goes to a CTU row, the others avoid CTU rows.  Returns the rows used."""
+    per = cv.W // 32
+    for i, s in enumerate(vspecs): cv.put(s, 0, 32 * (i % per) + 16, y0 + 4 * (i // per))
+    y = y0 + 4 * ((len(vspecs) + per - 1) // per)
+    ye = (y + 8 + 15) // 16 * 16
+    todo = {True: [s for s in hspecs if s.get("ctb")], False: [s for s in hspecs if not s.get("ctb")]}
+    end = y
+    while todo[True] or todo[False]:
+        row = todo[ye % cv.ctu == 0]
+        for i in range(min(len(row), cv.W // 4)): cv.put(row.pop(0), 1, 4 * i, ye)
+        end, ye = ye + 8, ye + 16
+    return end
+
+
+def _lf_blocks(extent, pattern):
+    """Blocks along one axis: `pattern` (sizes; ('sb', n): a CU of n coded in 8-sample sub-blocks) repeated until the extent is covered, the last block
+    cut to fit.  Returns the edges as (position, P length, Q length), derived as xSetMaxFilterLengthPQFromTransformSizes (LoopFilter.cpp:780) and
+    xSetMaxFilterLengthPQForCodingSubBlocks (:707) do, and the index of the (sub-)block every sample lies in."""
+    blocks, pos, i = [], 0, 0
+    while pos < extent:
+        it = pattern[i % len(pattern)]; i += 1
+        sb, n = (True, it[1]) if isinstance(it, tuple) else (False, it)
+        n = min(n, extent - pos)
+        blocks.append((pos, n, sb and n >= 16)); pos += n
+    edges, idx, k = [], np.zeros(extent, np.int64), 0
+    for j, (b0, n, sb) in enumerate(blocks):
+        if j:
+            a0, an, asb = blocks[j - 1]
+            P, Q = (1, 1) if min(an, n) <= 4 else (7 if an >= 32 else 3, 7 if n >= 32 else 3)
+            if asb: P = min(P, 5)
+            if sb: Q = min(Q, 5)
+            edges.append((b0, P, Q))
+        subs = range(b0, b0 + n, 8) if sb else [b0]
+        for s in subs:
+            if s > b0: edges.append((s, 2, 2) if s - b0 == 8 or s - b0 + 8 >= n else (s, 3, 3))
+            idx[s:b0 + n] = k; k += 1
+    return edges, idx
+
+
+def _lf_block_case(cv, xpat, ypat, t, qp=37, chroma_bs=(2, 1)):
+    """A picture of flat blocks (block (i, j) at level mid + t * ((i % 2) + (j % 3))) and the grids of their edges, every 4x4 unit of an edge with luma
+    Bs 2; chroma Bs alternates between the values of chroma_bs, and the chroma 'large' flag is set where both blocks are at least 16 luma samples."""
+    xe, xi = _lf_blocks(cv.W, xpat); ye, yi = _lf_blocks(cv.H, ypat)
+    mid = 1 << (cv.bd - 1)
+    Y = mid + t * ((xi[None, :] % 2) + (yi[:, None] % 3))
+    cv.planes[0][:, :cv.W] = Y
+    for c in (1, 2) if cv.chroma else ():
+        cv.planes[c][:, :cv.W >> 1] = Y[::2, ::2] - (c - 1) * t
+    size_at = lambda edges, extent: np.diff([0] + [e[0] for e in edges] + [extent])
+    for d, edges, other in ((0, xe, cv.H), (1, ye, cv.W)):
+        sizes = size_at(edges, cv.W if d == 0 else cv.H)
+        for k, (pos, P, Q) in enumerate(edges):
+            cb = chroma_bs[k % len(chroma_bs)]
+            sl = (slice(None), pos // 4) if d == 0 else (pos // 4, slice(None))
+            e = cv.lf[d][sl]
+            e["bs"] = 2 | (cb << 2) | (cb << 4)
+            e["len"] = 128 + (P << 4) + Q
+            e["flags"] = 32 if min(sizes[k], sizes[k + 1]) >= 16 else 0
+            e["qp"] = (qp, qp - 1, qp + 1)
+    return cv
+
+
+_LF_TIGHT = ([32, 4, 4, 4, 4, 8, 8, 8, 8, ("sb", 64), 32, 16, 8, 4, 4, 16, ("sb", 32), 32], [32, 8, 8, 4, 4, 8, 16, 32, ("sb", 32), 8, 8, 16, 32])
+
+
+def _lf_qp_specs(bd, ladf=None):
+    """Segments for one bit depth: for every Bs 1 / 2 and QP from -6 (bd - 8) to 63 (every 3rd), flat sides and a step sized so that a weak filter's delta
+    is about 2 tc (clipped to tc) and strong filtering fails; QP 63 with Bs 2 (tc index clipped at 65).  ladf: (level, qp) pairs, each a segment whose
+    LADF luma level is `level` exactly (P side level - k, Q side + k)."""
+    S, mid, pmax = [], 1 << (bd - 1), (1 << bd) - 1
+    pairs = ladf or [(None, qp) for qp in list(range(-6 * (bd - 8), 64, 3)) + [63]]
+    for lvl, qp in pairs:
+        for bs in (1, 2):
+            tc = lf_tc(_clip(0, 65, qp + 2 * (bs - 1)), bd)
+            t = _clip(2, pmax // 3, (32 * tc) // 6 + 2) // 2 * 2
+            v = (lvl if lvl is not None else mid) - t // 2
+            S.append(_lf_spec("any", dict(t=t), v=v, bs=bs, qp=qp))
+            S.append(_lf_spec("any", dict(t=-t), v=v + t, bs=bs, qp=qp))
+            S.append(_lf_spec("any", dict(t=t // 3, dp=1, dq=2), v=v, bs=bs, qp=qp))
+    return S
+
+
+def _lf_clip_specs(bd):
+    """Content at 0 and at the largest sample value with tc at its maximum (qp 63, Bs 2): the weak filter's result leaves [0, pmax] and is clipped; large
+    steps through the strong and long filters."""
+    pmax, S = (1 << bd) - 1, []
+    for flip in (False, True):
+        f = (lambda a: [pmax - x for x in a]) if flip else (lambda a: a)
+        p, q = [pmax - 95, pmax, pmax, pmax - 95, pmax - 95, pmax - 95, pmax - 95, pmax - 95], [pmax, pmax - 495, pmax - 990, pmax - 495] + [pmax - 495] * 4
+        S.append(dict(tag="weak11", qp=63, lines=[(f(p), f(q))] * 4, probes=[]))
+        p2 = [pmax - 300, pmax, pmax, pmax - 300] + [pmax - 300] * 4
+        S.append(dict(tag="weak01", qp=63, lines=[(f(p2), f(q))] * 4, probes=[]))
+    for lens, t in (((3, 3), 3000), ((7, 7), 3500), ((5, 3), 3900), ((7, 3), 2000)):
+        for flip in (False, True):
+            lo, hi = (0, t) if not flip else (pmax, pmax - t)
+            S.append(_lf_spec("any", dict(t=hi - lo), v=lo, lens=lens, qp=63))
+    return S
+
+
+def _lf_ctu_specs():
+    """Horizontal luma edges on CTU rows with a long P side, whose P side is run as length 3: the P side is flat for 4 rows and then steps by 40, so a
+    long P side would decide or filter differently."""
+    S = []
+    for (P, Q), tag in (((7, 7), "long37"), ((5, 7), "long37"), ((7, 5), "long35"), ((5, 5), "long35"), ((7, 3), "strong"), ((5, 3), "strong")):
+        s = _lf_spec(tag, dict(t=20), lens=(P, Q), qp=39, ctb=True)
+        for p, q in s["lines"]: p[4:] = [x + 40 for x in p[4:]]
+        S.append(s)
+    return S
+
+
+def _lf_slices(n, disable_every=5):
+    sl = np.zeros(n, LFSLICE_DTYPE)
+    for i in range(n):
+        sl[i]["beta"] = [((i + 5 * c) % 25) - 12 for c in range(3)]
+        sl[i]["tc"] = [((7 * i + 3 * c) % 25) - 12 for c in range(3)]
+        sl[i]["disable"] = i % disable_every == 3
+    return sl
+
+
+def _lf_ladf(bd):
+    """Five LADF intervals with shifts that take low QPs below 0, and (level, qp) pairs on each lower bound and one above it."""
+    s = abi.LfSeq(); s.ladfEnabled, s.ladfNumIntervals = 1, 5
+    sc = 1 << (bd - 8)
+    bounds, offs = [0, 40 * sc, 90 * sc, 140 * sc, 200 * sc], [-3, 4, -12, 7, -30]
+    for k in range(5): s.ladfQpOffset[k] = offs[k]; s.ladfIntervalLowerBound[k] = bounds[k]
+    pairs = [(lvl, qp) for b in bounds[1:] for lvl in (b, b + 1) for qp in (4, 30, 45)] + [(10 * sc, 20), (250 * sc, 20)]
+    return s, pairs
+
+
+def _lf_case(name):
+    kind, *a = LF_SWEEP_CASES[name]
+    if kind == "luma":
+        specs = lf_luma_specs()
+        cv = _LfCanvas(1024, 512, 10, 128)
+        used = _lf_layout(cv, specs, [dict(s) for s in specs])
+        assert used <= cv.H, used
+        return cv.case(name)
+    if kind == "chroma":
+        ctu, W, H = a
+        cv = _LfCanvas(W, H, 10, ctu)
+        hs = lf_chroma_specs(False) + [dict(s, ctb=True) for s in lf_chroma_specs(True)]
+        assert _lf_layout(cv, lf_chroma_specs(False), hs) <= H
+        return cv.case(name)
+    if kind == "qp":
+        bd, ladf = a
+        seq, pairs = _lf_ladf(bd) if ladf else (None, None)
+        specs = _lf_qp_specs(bd, pairs)
+        cv = _LfCanvas(512, 512 if not ladf else 256, bd, 32)
+        assert _lf_layout(cv, specs, [dict(s) for s in specs]) <= cv.H
+        # slices by CTU column: offsets 0, +12, -12 and mixed, for every component
+        sl = np.zeros(4, LFSLICE_DTYPE)
+        sl["beta"][1], sl["tc"][1] = 12, 12
+        sl["beta"][2], sl["tc"][2] = -12, -12
+        sl["beta"][3], sl["tc"][3] = (12, -12, 6), (-12, 12, -6)
+        nw, nh = cv.W // 32, cv.H // 32
+        cs = np.array([(i % nw) % 4 if not ladf else 0 for i in range(nw * nh)], np.uint8)
+        return cv.case(name, slices=sl if not ladf else None, ctu_slice=cs, seq=seq)
+    if kind == "clip":
+        cv = _LfCanvas(256, 128, 12, 128)
+        specs = _lf_clip_specs(12)
+        assert _lf_layout(cv, specs, [dict(s) for s in specs]) <= cv.H
+        return cv.case(name)
+    if kind == "blocks":
+        W, H, bd, ctu, chroma, strides, xpat, ypat, t, nsl = a
+        cv = _lf_block_case(_LfCanvas(W, H, bd, ctu, chroma, strides), xpat, ypat, t)
+        if nsl <= 1: return cv.case(name, classify=W * H <= 1 << 20)
+        nctu = ((W + ctu - 1) // ctu) * ((H + ctu - 1) // ctu)
+        cs = np.array([(37 * i) % nsl for i in range(nctu)], np.uint8)
+        return cv.case(name, slices=_lf_slices(nsl), ctu_slice=cs)
+    if kind == "ctu":
+        ctu, W, H = a
+        cv = _LfCanvas(W, H, 10, ctu)
+        specs = _lf_ctu_specs()
+        _lf_layout(cv, [], specs * (W // 4 // len(specs)), y0=ctu - 16)
+        return cv.case(name)
+    raise KeyError(name)
+
+
+LF_SWEEP_CASES = {
+    "luma_decisions_10bit": ("luma",),
+    "chroma_decisions_10bit": ("chroma", 128, 256, 320),
+    "chroma_ctb_ctu32": ("chroma", 32, 256, 320),
+    "chroma_ctb_ctu64": ("chroma", 64, 256, 320),
+    "qp_extremes_8bit": ("qp", 8, False), "qp_extremes_9bit": ("qp", 9, False), "qp_extremes_10bit": ("qp", 10, False), "qp_extremes_12bit": ("qp", 12, False),
+    "qp_ladf_10bit": ("qp", 10, True), "qp_ladf_12bit": ("qp", 12, True),
+    "clipping_12bit": ("clip",),
+    "tight_spacing": ("blocks", 512, 256, 10, 128, 1, None, *_LF_TIGHT, 12, 1),
+    "ctu_rows_ctu32": ("ctu", 32, 256, 64), "ctu_rows_ctu64": ("ctu", 64, 256, 128), "ctu_rows_ctu128": ("ctu", 128, 256, 256),
+    "ctu_edges_ctu32_200x136": ("blocks", 200, 136, 10, 32, 1, None, [8, 8, 16, 32, 4, 4, 8, 16], [32, 16, 8, 8, 32, ("sb", 32)], 12, 1),
+    "ctu_edges_ctu64_416x240": ("blocks", 416, 240, 10, 64, 1, None, [32, 32, 16, 16, 32, ("sb", 64), 64], [64, 32, 16, 16, ("sb", 32), 32], 12, 1),
+    "ctu_edges_ctu128_1928x1080": ("blocks", 1928, 1080, 10, 128, 1, None, [64, 64, 32, 32, 16, 16, 8, 8, 4, 4, 8, 8, 16, 32, ("sb", 64), 32, 32],
+                                   [128, 64, 32, 32, 64, 16, 16, 32], 12, 1),
+    "slices_64": ("blocks", 512, 128, 10, 32, 1, None, *_LF_TIGHT, 12, 64),
+    "geometry_400_8bit": ("blocks", 256, 128, 8, 64, 0, None, *_LF_TIGHT, 4, 1),
+    "geometry_400_stride": ("blocks", 256, 128, 10, 128, 0, (264, 0, 0), *_LF_TIGHT, 12, 1),
+    "geometry_strides": ("blocks", 256, 128, 10, 128, 1, (263, 133, 140), *_LF_TIGHT, 12, 1),
+    "uhd_3840x2160": ("blocks", 3840, 2160, 10, 128, 1, None, *_LF_TIGHT, 12, 1),
+}
+
+_lf_sweep_cache = {}
+
+
+def lf_sweep(name):
+    """One case of the designed K3 sweep (LF_SWEEP_CASES) as a dict: geometry (g, W, H, bd, ctu, chroma, strides), the planes (stride padding holds -7),
+    the grids lfV / lfH, ctuSlice (None: every CTU in slice 0), the slice table, the LfSeq, and segs: the designed segments (dir, comp, x, y in the
+    component's plane, the tag the decision is designed to take ('any': content for the comparisons only) and probes (quantity, threshold, offset):
+    lf_decisions' q[quantity] - q[threshold] == offset).  classify: whether the picture is small enough to classify every segment in Python."""
+    if name not in _lf_sweep_cache: _lf_sweep_cache[name] = _lf_case(name)
+    c = _lf_sweep_cache[name]
+    return dict(c, planes=[None if p is None else p.copy() for p in c["planes"]])
