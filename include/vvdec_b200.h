@@ -167,7 +167,11 @@ typedef struct b200_vb {  /* ph virtual boundaries (PicHeader), luma sample posi
   int32_t posX[3], posY[3];
 } b200_vb;
 
-/* Kernel-level K4: src planes -> dst planes (both host; dst must be a different buffer). vb may be NULL. */
+/* Kernel-level K4: src planes -> dst planes (both host; dst must be a different buffer). vb may be NULL.  Only the plane width of each dst row is
+ * written: the stride padding keeps what the caller put there.  Returns B200_ERR_PARAM, before any device work and with dst untouched, for a
+ * chromaFormat other than 0 (4:0:0) or 1 (4:2:0), a CTU size other than 32 / 64 / 128, a bit depth outside 8..12, a width or height that is not a
+ * multiple of 8, a plane stride below its plane's width or not a multiple of 4 (Cr included), a type other than 0..4 or B200_SAO_OFF, a BO band above
+ * 31, more than 3 vertical or horizontal virtual boundaries, or a virtual boundary that is not a multiple of 8 strictly inside the picture. */
 B200_API int b200_sao_picture(const b200_geom* g, const int16_t* const src[3], int16_t* const dst[3],
                               const b200_sao_ctu* ctus, const b200_vb* vb);
 
@@ -205,6 +209,13 @@ typedef struct b200_alf_tables {
   int32_t        numCc[2];
 } b200_alf_tables;
 
+/* Kernel-level K5: src planes -> dst planes (both host).  Only the plane width of each dst row is written.  Returns B200_ERR_PARAM, before any device
+ * work and with dst untouched, for the geometry b200_sao_picture refuses, a bit depth above 10 (ALF is defined for 8, 9 and 10 bit), numLumaSets
+ * outside 16..24, a negative numChromaAlts or numCc (tables may hold several slices' APS filters), and for a CTU record with an enable bit outside the defined ones, lumaSet >=
+ * numLumaSets (luma on), chromaAlt >= numChromaAlts (that chroma component on), ccIdx > numCc, PAD_TL together with CLIP_TOP or CLIP_LEFT or on the
+ * picture's first CTU row or column, PAD_BR together with CLIP_BOTTOM or CLIP_RIGHT or on the last CTU row or column, or PAD_WIDE on a component
+ * whose ccIdx is not 0.  The picture path (B200_PIC_ALF) refuses the same records in b200_pic_run, ALF above 10 bit in b200_pic_upload, and SAO or
+ * ALF on a context whose plane strides are not all multiples of 4. */
 B200_API int b200_alf_picture(const b200_geom* g, const int16_t* const src[3], int16_t* const dst[3],
                               const b200_alf_ctu* ctus, const b200_alf_tables* tabs);
 

@@ -42,10 +42,12 @@ def test_filter_flatteners_round_trip(ref, W, H, ctu):
 
 
 @pytest.mark.parametrize("seed,kw", [(1, dict()), (2, dict(ctu=32, bd=8)), (3, dict(ctu=64, slice_type=2, isp=30)), (4, dict(affine=60, split=85)),
-                                     (5, dict(tools=None, slices=3, ctu=32))])
+                                     (5, dict(tools=None, slices=3, ctu=32)),
+                                     (6, dict(slices=3, lf_across_slices=False))])
 def test_flattened_deblocking_grids_are_legal(ref, seed, kw):
     """The grids the glue flattens from the reference's own calcFilterStrengths (sub-block lengths 5 and 2 of affine / SbTMVP CUs, 4-wide CUs, CTU 32
-    rows, intra pictures) meet the rule of the flat pass: the picture path runs them without checking."""
+    rows, intra pictures) meet the rule of the flat pass: the picture path runs them without checking.  Its SAO / ALF records, clip and pad flags of
+    slices that do not filter across each other included, meet the rule of b200_sao_picture / b200_alf_picture."""
     from tests import helpers
     case = helpers.SeamCase(ref, np.random.default_rng(seed), 416, 240, **kw)
     pic, rc = case.flatten()
@@ -53,5 +55,12 @@ def test_flattened_deblocking_grids_are_legal(ref, seed, kw):
     W4, H4 = case.W // 4, case.H // 4
     lfV, lfH = pic["lfV"].reshape(H4, W4), pic["lfH"].reshape(H4, W4)
     assert synth.lf_grid_problems(lfV, 0, case.g) == [] and synth.lf_grid_problems(lfH, 1, case.g) == []
+    # the SAO / ALF records the glue flattens meet the rule b200_sao_picture / b200_alf_picture enforce, which the picture path shares
+    st = pic["struct"]
+    if st.flags & abi.PIC_SAO: assert synth.k45_record_problems("sao", case.g, pic["sao"]) == []
+    if st.flags & abi.PIC_ALF:
+        T = pic["alfTabs"]
+        t = dict(lumaCoeff=pic["alfArrays"]["lumaCoeff"].reshape(-1, 4, 25, 13), chromaCoeff=np.zeros((T.numChromaAlts, 7)), cc=[np.zeros((T.numCc[c], 7)) for c in range(2)])
+        assert synth.k45_record_problems("alf", case.g, pic["alf"]["ctus"], t) == []
     lens = {int(v) >> 4 & 7 for v in lfV["len"][lfV["bs"] & 3 > 0]} | {int(v) & 7 for v in lfV["len"][lfV["bs"] & 3 > 0]}
     assert lens >= {1, 3}, lens

@@ -435,3 +435,67 @@ def test_designed_deblocking_in_a_picture(b200, oracle, name, strides):
             assert len(bad) == 0, f"{name}: plane {c}: {len(bad)} diffs, first at {bad[:1].tolist()}"
     finally:
         b200.b200_ctx_destroy(ctx)
+
+
+def _filter_picture(b200, oracle, case, strides, sao, alf, flags=abi.PIC_SAO | abi.PIC_ALF, bd=None):
+    """A designed K4 / K5 sweep picture through b200_decompress_picture: its planes as `given`, no PUs or TUs, SAO and / or ALF on with the given
+    records.  Returns the handle's error (or None) and, when it decoded, whether the frame equals the oracle chain's on the plane width."""
+    W, H, ctu = case["W"], case["H"], case["ctu"]
+    bd = bd or case["bd"]
+    g = abi.make_geom(W, H, bd, ctu=ctu, strides=strides)
+    given = []
+    for c in range(3):
+        w, h = (W, H) if c == 0 else (W // 2, H // 2)
+        p = np.zeros((h, g.stride[c]), np.int16); p[:, :w] = case["planes"][c][:, :w]; given.append(p)
+    pic = synth.gen_picture(np.random.default_rng(3), W, H, bd, ctu=ctu, dst_slot=4, inter=False, tu_kw=dict(p_cbf=0.0), deblock=False, sao=False, alf=False)
+    st = pic["struct"]
+    pic["given"] = given
+    for c in range(3): st.given[c] = given[c].ctypes.data
+    T = abi.make_alf_tables(alf)
+    pic["sao"], pic["alf"], pic["alfTabs"] = sao, dict(ctus=alf["ctus"]), T
+    st.flags |= flags; st.sao = sao.ctypes.data; st.alf = alf["ctus"].ctypes.data; st.alfTabs = C.addressof(T)
+    ctx = C.c_void_p()
+    vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 2, -1))
+    try:
+        h = b200.b200_decompress_picture(ctx, C.byref(st))
+        if h < 0: return b200.b200_last_error(), None
+        vvdec_b200.check(b200.b200_wait_picture(ctx, h, None, 0))
+        got = [np.zeros_like(p) for p in given]
+        vvdec_b200.check(b200.b200_get_frame(ctx, 4, abi.plane_ptrs(got)))
+    finally:
+        b200.b200_ctx_destroy(ctx)
+    want, _ = oracle_decompress(oracle, g, [[np.zeros_like(p) for p in given] for _ in range(4)], pic)
+    for c in range(3):
+        w, hh = (W, H) if c == 0 else (W // 2, H // 2)
+        bad = np.argwhere(want[c][:hh, :w] != got[c][:hh, :w])
+        if len(bad): return None, f"{case['name']}: plane {c}: {len(bad)} diffs, first at {bad[:1].tolist()}"
+    return None, True
+
+
+@pytest.mark.parametrize("kind,name,strides", [("alf", "ccalf_10bit_ctu32", None), ("alf", "coeffs_10bit_ctu32_last24", (280, 136, 140)),
+                                               ("sao", "avail_masks_ctu32", None)])
+def test_designed_sao_alf_in_a_picture(b200, oracle, kind, name, strides):
+    """Cases of the designed K4 / K5 sweeps through b200_decompress_picture with SAO and ALF on: CC-ALF clipping both ways; CTU 32 with the ALF virtual
+    boundary rows at the picture bottom and padded strides; every SAO avail mask.  The other filter's records come from gen_sao / gen_alf.  The frame
+    equals the oracle chain's."""
+    rng = np.random.default_rng(11)
+    case = synth.alf_sweep(name) if kind == "alf" else synth.sao_sweep(name)
+    W, H, ctu = case["W"], case["H"], case["ctu"]
+    sao = case["ctus"] if kind == "sao" else synth.gen_sao(rng, W, H, ctu, case["bd"], p_on=0.5)
+    alf = case["tables"] if kind == "alf" else synth.gen_alf(rng, W, H, ctu, case["bd"], n_aps=2)
+    err, ok = _filter_picture(b200, oracle, case, strides, sao, alf)
+    assert err is None and ok is True, (err, ok)
+
+
+@pytest.mark.parametrize("what,bad,fixed", [("ALF at 12 bit", dict(bd=12), dict(bd=10)), ("SAO with a Cb stride of 4k + 2", dict(strides=(264, 134, 132)), dict(strides=(264, 136, 132)))])
+def test_sao_alf_picture_refusals(b200, oracle, what, bad, fixed):
+    """b200_decompress_picture refuses ALF above 10 bit and SAO / ALF with a plane stride that is not a multiple of 4 before any device work; the same
+    picture with the field fixed decodes and equals the oracle chain's."""
+    case = synth.sao_sweep("eo_8bit_ctu32_partial")
+    rng = np.random.default_rng(12)
+    alf = synth.gen_alf(rng, case["W"], case["H"], case["ctu"], 10, n_aps=2)
+    flags = abi.PIC_ALF if "bd" in bad else abi.PIC_SAO
+    err, ok = _filter_picture(b200, oracle, case, bad.get("strides"), case["ctus"], alf, flags=flags, bd=bad.get("bd", 10))
+    assert err is not None and b"b200_pic_upload" in err, (what, err, ok)
+    err, ok = _filter_picture(b200, oracle, case, fixed.get("strides"), case["ctus"], alf, flags=flags, bd=fixed.get("bd", 10))
+    assert err is None and ok is True, (what, err, ok)

@@ -197,6 +197,76 @@ B200_API int b200_lf_deblock(const b200_geom* g, int16_t* const planes[3], const
   return 0;
 }
 
+// The geometry K4 and K5 filter (include/vvdec_b200.h): 4:0:0 or 4:2:0, CTU 32 / 64 / 128, a picture of whole 8x8 units, and every plane's stride at
+// least its width and a multiple of 4 (both kernels move 4 samples per 8-byte access, Cr included).  Returns false with the error set.
+static bool k45_geom_ok(const char* fn, const b200_geom& g, int maxBitDepth)
+{
+  if (g.chromaFormat != 0 && g.chromaFormat != 1) { set_error("%s: chromaFormat %d (only 0 = 4:0:0 and 1 = 4:2:0)", fn, g.chromaFormat); return false; }
+  if (g.ctuSize != 32 && g.ctuSize != 64 && g.ctuSize != 128) { set_error("%s: CTU size %d (32, 64 or 128)", fn, g.ctuSize); return false; }
+  if (g.bitDepth < 8 || g.bitDepth > maxBitDepth) { set_error("%s: bit depth %d (8..%d)", fn, g.bitDepth, maxBitDepth); return false; }
+  if (g.width <= 0 || g.height <= 0 || (g.width & 7) || (g.height & 7)) { set_error("%s: picture %dx%d is not a multiple of 8", fn, g.width, g.height); return false; }
+  for (int c = 0; c < (g.chromaFormat ? 3 : 1); c++) {
+    const int pw = c ? g.width >> 1 : g.width;
+    if (g.stride[c] < pw || (g.stride[c] & 3)) { set_error("%s: plane %d stride %d (at least the plane width %d, a multiple of 4)", fn, c, g.stride[c], pw); return false; }
+  }
+  return true;
+}
+
+// SAO records and virtual boundaries: types 0..4 or OFF, BO bands 0..31, at most 3 boundaries per direction on the 8x8 grid strictly inside the picture.
+static bool sao_records_ok(const b200_geom& g, const b200_sao_ctu* ctus, const b200_vb* vb)
+{
+  const size_t nCtu = (size_t)((g.width + g.ctuSize - 1) / g.ctuSize) * ((g.height + g.ctuSize - 1) / g.ctuSize);
+  for (size_t i = 0; i < nCtu; i++)
+    for (int c = 0; c < (g.chromaFormat ? 3 : 1); c++) {
+      const int t = ctus[i].type[c];
+      if (t != B200_SAO_OFF && t > B200_SAO_BO) { set_error("b200_sao_picture: CTU %zu component %d: type %d", i, c, t); return false; }
+      if (t == B200_SAO_BO && ctus[i].band[c] > 31) { set_error("b200_sao_picture: CTU %zu component %d: band %d", i, c, ctus[i].band[c]); return false; }
+    }
+  if (!vb) return true;
+  if (vb->numVer < 0 || vb->numVer > 3 || vb->numHor < 0 || vb->numHor > 3) { set_error("b200_sao_picture: %d / %d virtual boundaries (0..3 each)", vb->numVer, vb->numHor); return false; }
+  for (int k = 0; k < vb->numVer; k++)
+    if (vb->posX[k] <= 0 || vb->posX[k] >= g.width || (vb->posX[k] & 7)) { set_error("b200_sao_picture: vertical virtual boundary at x = %d", vb->posX[k]); return false; }
+  for (int k = 0; k < vb->numHor; k++)
+    if (vb->posY[k] <= 0 || vb->posY[k] >= g.height || (vb->posY[k] & 7)) { set_error("b200_sao_picture: horizontal virtual boundary at y = %d", vb->posY[k]); return false; }
+  return true;
+}
+
+// ALF tables and records: every index inside its table, no undefined enable bit, and the padding forms the reference can produce (a corner is padded only
+// where both adjacent sides are readable and the diagonal CTU exists; the wide chroma form only without CC-ALF on that component).
+static bool alf_records_ok(const b200_geom& g, const b200_alf_ctu* ctus, const b200_alf_tables& T)
+{
+  const char* fn = "b200_alf_picture";
+  if (T.numLumaSets < 16 || T.numLumaSets > 24) { set_error("%s: numLumaSets %d (16..24)", fn, T.numLumaSets); return false; }
+  // the tables of a picture with several slices hold every slice's APS filters, so only the lower bounds are fixed
+  if (T.numChromaAlts < 0) { set_error("%s: numChromaAlts %d", fn, T.numChromaAlts); return false; }
+  for (int c = 0; c < 2; c++) if (T.numCc[c] < 0) { set_error("%s: numCc[%d] %d", fn, c, T.numCc[c]); return false; }
+  const int ctusW = (g.width + g.ctuSize - 1) / g.ctuSize, ctusH = (g.height + g.ctuSize - 1) / g.ctuSize;
+  for (int i = 0; i < ctusW * ctusH; i++) {
+    const b200_alf_ctu& a = ctus[i];
+    const int cx = i % ctusW, cy = i / ctusW, f = a.enable[0];
+    if ((f & ~0x7f) || (a.enable[1] & ~3) || (a.enable[2] & ~3)) { set_error("%s: CTU %d: undefined enable bits %02x %02x %02x", fn, i, a.enable[0], a.enable[1], a.enable[2]); return false; }
+    if ((f & 1) && a.lumaSet >= T.numLumaSets) { set_error("%s: CTU %d: lumaSet %d of %d", fn, i, a.lumaSet, T.numLumaSets); return false; }
+    for (int c = 0; c < 2; c++) {
+      if ((a.enable[1 + c] & 1) && a.chromaAlt[c] >= T.numChromaAlts) { set_error("%s: CTU %d: chromaAlt[%d] %d of %d", fn, i, c, a.chromaAlt[c], T.numChromaAlts); return false; }
+      if (a.ccIdx[c] > T.numCc[c]) { set_error("%s: CTU %d: ccIdx[%d] %d of %d", fn, i, c, a.ccIdx[c], T.numCc[c]); return false; }
+      if ((a.enable[1 + c] & B200_ALF_PAD_WIDE) && a.ccIdx[c]) { set_error("%s: CTU %d: PAD_WIDE with CC-ALF on component %d", fn, i, c + 1); return false; }
+    }
+    if ((f & B200_ALF_PAD_TL) && ((f & (B200_ALF_CLIP_TOP | B200_ALF_CLIP_LEFT)) || !cx || !cy)) { set_error("%s: CTU %d: PAD_TL with a clipped top / left side or on the picture's first CTU row / column", fn, i); return false; }
+    if ((f & B200_ALF_PAD_BR) && ((f & (B200_ALF_CLIP_BOTTOM | B200_ALF_CLIP_RIGHT)) || cx == ctusW - 1 || cy == ctusH - 1)) { set_error("%s: CTU %d: PAD_BR with a clipped bottom / right side or on the picture's last CTU row / column", fn, i); return false; }
+  }
+  return true;
+}
+
+// dst planes of the kernel-level filters: only the plane width of each row goes back, so the caller's stride padding keeps what it held
+static int download_plane_rows(const b200_geom* g, int16_t* const planes[3], const DevPlanes& dp, cudaStream_t s)
+{
+  for (int c = 0; c < (g->chromaFormat ? 3 : 1); c++) {
+    const size_t pitch = (size_t)g->stride[c] * sizeof(int16_t);
+    B200_CUDA(cudaMemcpy2DAsync(planes[c], pitch, dp.p[c], pitch, (size_t)(c ? g->width >> 1 : g->width) * sizeof(int16_t), c ? g->height >> 1 : g->height, cudaMemcpyDeviceToHost, s));
+  }
+  return 0;
+}
+
 static int upload_src_alloc_dst(const b200_geom* g, const int16_t* const src[3], DevPlanes& ds, DevPlanes& dd, cudaStream_t s)
 {
   const int nPlanes = g->chromaFormat ? 3 : 1;
@@ -214,7 +284,7 @@ static int upload_src_alloc_dst(const b200_geom* g, const int16_t* const src[3],
 B200_API int b200_sao_picture(const b200_geom* g, const int16_t* const src[3], int16_t* const dst[3], const b200_sao_ctu* ctus, const b200_vb* vb)
 {
   B200_CHECK(g && src && dst && ctus, "b200_sao_picture: null argument");
-  B200_CHECK((g->width & 7) == 0 && (g->stride[0] & 3) == 0 && (!g->chromaFormat || (g->stride[1] & 3) == 0), "b200_sao_picture: width must be a multiple of 8, strides of 4");
+  if (!k45_geom_ok("b200_sao_picture", *g, 12) || !sao_records_ok(*g, ctus, vb)) return B200_ERR_PARAM;
   if (int rc = ensure_device()) return rc;
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
@@ -226,7 +296,7 @@ B200_API int b200_sao_picture(const b200_geom* g, const int16_t* const src[3], i
   B200_CUDA(cudaMemcpyAsync(g_hw.misc[0].p, ctus, nCtu * sizeof(b200_sao_ctu), cudaMemcpyHostToDevice, s));
   L.ctus = g_hw.misc[0].as<b200_sao_ctu>();
   if (int rc = launch_sao(L, s)) return rc;
-  if (int rc = download_planes(g, dst, L.dst, s)) return rc;
+  if (int rc = download_plane_rows(g, dst, L.dst, s)) return rc;
   B200_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
@@ -300,8 +370,8 @@ B200_API int b200_intra_predict(const b200_geom* g, int16_t* const planes[3], co
 B200_API int b200_alf_picture(const b200_geom* g, const int16_t* const src[3], int16_t* const dst[3], const b200_alf_ctu* ctus, const b200_alf_tables* T)
 {
   B200_CHECK(g && src && dst && ctus && T, "b200_alf_picture: null argument");
-  B200_CHECK((g->width & 7) == 0 && (g->stride[0] & 3) == 0 && (!g->chromaFormat || (g->stride[1] & 3) == 0), "b200_alf_picture: width must be a multiple of 8, strides of 4");
-  B200_CHECK(T->numLumaSets >= 16 && T->numLumaSets <= 24, "b200_alf_picture: numLumaSets %d", T->numLumaSets);
+  // ALF is defined up to 10 bit (the reference's AdaptiveLoopFilter::create refuses more, and its clipping values exist for 8, 9 and 10 bit only)
+  if (!k45_geom_ok("b200_alf_picture", *g, 10) || !alf_records_ok(*g, ctus, *T)) return B200_ERR_PARAM;
   if (int rc = ensure_device()) return rc;
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
@@ -325,7 +395,7 @@ B200_API int b200_alf_picture(const b200_geom* g, const int16_t* const src[3], i
   L.ctus = g_hw.misc[0].as<b200_alf_ctu>();
   StreamSet ss(s);
   if (int rc = launch_alf(L, ss)) return rc;
-  if (int rc = download_planes(g, dst, L.dst, s)) return rc;
+  if (int rc = download_plane_rows(g, dst, L.dst, s)) return rc;
   B200_CUDA(cudaStreamSynchronize(s));
   return 0;
 }

@@ -190,7 +190,9 @@ size_t mc_tile_capacity(const b200_geom& g, size_t numPus)
 }
 
 // Per-CTU side information (SAO / ALF / slice index): every index the filter kernels use to address a table is range-checked here
-// (error bit 4 of the PU meta block), so that a malformed record cannot make them read outside the uploaded arrays.
+// (error bit 4 of the PU meta block), so that a malformed record cannot make them read outside the uploaded arrays.  ALF records also follow the
+// rule b200_alf_picture checks on the host: no undefined enable bit, PAD_TL / PAD_BR only with both adjacent sides readable and inside the CTU grid,
+// PAD_WIDE only without CC-ALF on that component.
 __global__ void __launch_bounds__(256) ctu_validate_kernel(const b200_sao_ctu* __restrict__ sao, const b200_alf_ctu* __restrict__ alf, const uint8_t* __restrict__ ctuSlice,
                                                            int nCtu, const CtuLimits lim, int* meta)
 {
@@ -201,7 +203,15 @@ __global__ void __launch_bounds__(256) ctu_validate_kernel(const b200_sao_ctu* _
   if (alf) {
     const b200_alf_ctu a = alf[i];
     if ((a.enable[0] & 1) && a.lumaSet >= lim.numLumaSets) ok = false;
-    for (int c = 0; c < 2; c++) { if ((a.enable[1 + c] & 1) && a.chromaAlt[c] >= lim.numChromaAlts) ok = false; if (a.ccIdx[c] > lim.numCc[c]) ok = false; }
+    for (int c = 0; c < 2; c++) {
+      if ((a.enable[1 + c] & 1) && a.chromaAlt[c] >= lim.numChromaAlts) ok = false;
+      if (a.ccIdx[c] > lim.numCc[c]) ok = false;
+      if ((a.enable[1 + c] & ~3) || ((a.enable[1 + c] & B200_ALF_PAD_WIDE) && a.ccIdx[c])) ok = false;
+    }
+    const int f = a.enable[0], cx = i % lim.ctusW, cy = i / lim.ctusW;
+    if (f & ~0x7f) ok = false;
+    if ((f & B200_ALF_PAD_TL) && ((f & (B200_ALF_CLIP_TOP | B200_ALF_CLIP_LEFT)) || !cx || !cy)) ok = false;
+    if ((f & B200_ALF_PAD_BR) && ((f & (B200_ALF_CLIP_BOTTOM | B200_ALF_CLIP_RIGHT)) || cx == lim.ctusW - 1 || cy == lim.ctusH - 1)) ok = false;
   }
   if (ctuSlice && ctuSlice[i] >= lim.numLfSlices) ok = false;
   if (!ok) atomicOr(&meta[LM_ERR], 4);

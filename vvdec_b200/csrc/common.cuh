@@ -98,7 +98,7 @@ constexpr int K1_LISTS = 4;      // TU max dimension <= 8, 16, 32, 64
 constexpr int LM_CNT = 0, LM_OFF = 32, LM_CUR = 64, LM_DONE = 96, LM_ERR = 97, LM_INTS = 128;   // meta layout: counts, offsets, cursors, ticket, error bits
 int launch_mc_bucket(const b200_pu* pus, size_t numPus, uint32_t* tiles, size_t capTiles, int* meta, const b200_geom& g, int numSlots, int numWp, size_t numDmvr, cudaStream_t s);
 int launch_tu_bucket(const b200_tu* tus, size_t numTus, uint32_t* idx, int* meta, const b200_geom& g, size_t numCoefs, size_t numScaling, cudaStream_t s);
-struct CtuLimits { int numLumaSets, numChromaAlts, numCc[2], numLfSlices; };
+struct CtuLimits { int numLumaSets, numChromaAlts, numCc[2], numLfSlices, ctusW, ctusH; };
 int launch_ctu_validate(const b200_sao_ctu* sao, const b200_alf_ctu* alf, const uint8_t* ctuSlice, int nCtu, const CtuLimits& lim, int* meta, cudaStream_t s);   // after launch_mc_bucket (same meta block)
 size_t mc_tile_capacity(const b200_geom& g, size_t numPus);
 int num_sms();                   // SM count of the current device (persistent-style grids are sized from it)

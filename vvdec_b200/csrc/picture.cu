@@ -151,6 +151,10 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   B200_CHECK(!(p->flags & B200_PIC_DEBLOCK) || (p->lfV && p->lfH && p->lfSlices && p->numLfSlices >= 1 && p->numLfSlices <= 64), "b200_pic_upload: deblocking data missing");
   B200_CHECK(!(p->flags & B200_PIC_SAO) || p->sao, "b200_pic_upload: SAO data missing");
   B200_CHECK(!(p->flags & B200_PIC_ALF) || (p->alf && p->alfTabs && p->alfTabs->numLumaSets >= 16), "b200_pic_upload: ALF data missing");
+  B200_CHECK(!(p->flags & B200_PIC_ALF) || c->g.bitDepth <= 10, "b200_pic_upload: ALF at bit depth %d (ALF is defined up to 10 bit)", c->g.bitDepth);
+  // K4 and K5 move 4 samples per 8-byte access on every plane
+  B200_CHECK(!(p->flags & (B200_PIC_SAO | B200_PIC_ALF)) || (!(c->g.stride[0] & 3) && (!c->g.chromaFormat || (!(c->g.stride[1] & 3) && !(c->g.stride[2] & 3)))),
+             "b200_pic_upload: SAO / ALF need every plane stride to be a multiple of 4 (strides %d, %d, %d)", c->g.stride[0], c->g.stride[1], c->g.stride[2]);
   B200_CHECK(p->numPus < (1u << 26) && p->numTus < (1u << 31), "b200_pic_upload: too many records");
   B200_CHECK(p->numWp >= 0 && p->numWp <= 255 && (p->wp || !p->numWp), "b200_pic_upload: weighted-prediction table (at most 255 entries)");
   B200_CHECK(!(p->flags & B200_PIC_LMCS) || (p->lmcs && p->lmcs->invLUT && (!p->lmcs->chromaAdj || p->lmcs->vpdus) && p->lmcs->orgCW == (1 << c->g.bitDepth) / 16), "b200_pic_upload: LMCS data missing or inconsistent");
@@ -260,6 +264,7 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
     CtuLimits lim; const bool alfOn = p->flags & B200_PIC_ALF;
     lim.numLumaSets = alfOn ? T->numLumaSets : 0; lim.numChromaAlts = alfOn ? T->numChromaAlts : 0; lim.numCc[0] = alfOn ? T->numCc[0] : 0; lim.numCc[1] = alfOn ? T->numCc[1] : 0;
     lim.numLfSlices = p->numLfSlices;
+    lim.ctusW = (g.width + g.ctuSize - 1) / g.ctuSize; lim.ctusH = (g.height + g.ctuSize - 1) / g.ctuSize;
     const bool any = (p->flags & (B200_PIC_SAO | B200_PIC_ALF)) || ((p->flags & B200_PIC_DEBLOCK) && p->ctuSlice);
     if (int rc = launch_ctu_validate((p->flags & B200_PIC_SAO) ? A.sao : nullptr, alfOn ? A.alf : nullptr, (p->flags & B200_PIC_DEBLOCK) ? A.ctuSlice : nullptr, (int)nCtu, lim, A.mcMeta, s)) return rc;
     if (any) c->launches += 1;
@@ -282,7 +287,7 @@ B200_API int b200_pic_run(b200_ctx* c, int ai)
   B200_CHECK(!(A.hMeta[LM_ERR] & 1), "b200_pic_run: the picture's PU list holds an invalid record (reference slots, block size or flag combination)");
   B200_CHECK(!(A.hMeta[LM_ERR] & 2), "b200_pic_run: more MC tiles than the picture can hold (overlapping PUs?)");
   B200_CHECK(!(A.hMeta[LM_ERR] & 8), "b200_pic_run: an intra block record is invalid (geometry, mode, or availability reaching outside the picture)");
-  B200_CHECK(!(A.hMeta[LM_ERR] & 4), "b200_pic_run: a CTU record (SAO type / band, ALF filter index, slice index) is out of range");
+  B200_CHECK(!(A.hMeta[LM_ERR] & 4), "b200_pic_run: a CTU record (SAO type / band, ALF filter index or clip / pad flags, slice index) is out of range");
   B200_CHECK(!A.hMeta[LM_INTS + LM_ERR], "b200_pic_run: the picture's TU list holds an invalid record");
   B200_CUDA(cudaStreamWaitEvent(s, A.uploaded, 0));
   const b200_geom& g = c->g;

@@ -1816,3 +1816,389 @@ def lf_sweep(name):
     if name not in _lf_sweep_cache: _lf_sweep_cache[name] = _lf_case(name)
     c = _lf_sweep_cache[name]
     return dict(c, planes=[None if p is None else p.copy() for p in c["planes"]])
+
+
+# ---- K4 / K5: the designed SAO and ALF sweep ----------------------------------------------------------------------------------------------------------
+def sao_max_offset(bd):
+    """The largest legal SAO offset magnitude: (1 << (min(bd, 10) - 5)) - 1, scaled by 1 << (bd - min(bd, 10)): 7, 15, 31, 31, 62, 124 at 8..12 bit."""
+    b = min(bd, 10)
+    return ((1 << (b - 5)) - 1) << (bd - b)
+
+
+def alf_clip_values(bd):
+    """m_alfClippVls: the clipping value of clip index 0..3."""
+    return [1 << bd, 1 << (bd - 3), 1 << (bd - 5), 1 << (bd - 7)]
+
+
+def _k45_planes(W, H, chroma, strides, content):
+    """Planes (stride padding holds -7) with content(c, w, h) -> (h, w) samples."""
+    out = []
+    for c in range(3 if chroma else 1):
+        w, h = (W, H) if c == 0 else (W // 2, H // 2)
+        p = np.full((h, strides[c] if strides else w), -7, np.int16)
+        p[:, :w] = content(c, w, h)
+        out.append(p)
+    return out
+
+
+def alf_class_sums(plane, bd, ctu):
+    """Restates the ALF luma classification only (deriveClassificationBlk, AdaptiveLoopFilter.cpp:969) for every 4x4 block of `plane` (h, w), picture
+    borders replicated as prepareCTU does, the CTU virtual boundary at vbPos = ctu - 4.  Returns (h/4, w/4) arrays sV, sH, sD0, sD1, act, cls, tr, vb
+    (the block lies at vbPos - 4 or vbPos: x96 activity and one row pair skipped) and cmp / nz, (5, h/4, w/4): the sign of sV - sH, sD0 - sD1,
+    d1*hv0 - hv1*d0, hvd1 - 2*hvd0, 2*hvd1 - 9*hvd0 and whether the larger side of that comparison is nonzero."""
+    h, w = plane.shape
+    P = np.pad(plane.astype(np.int64), 4, mode="edge")
+    vbPos = ctu - 4
+    by, bx = np.arange(h // 4) * 4, np.arange(w // 4) * 4
+    above, below = by % ctu == vbPos - 4, by % ctu == vbPos
+
+    def p(yy, xx):
+        return P[yy[:, None] + 4, xx[None, :] + 4]
+    S = np.zeros((4, len(by), len(bx)), np.int64)
+    for r in range(4):
+        Y = by - 2 + 2 * r
+        up = np.where((Y > 0) & (Y % ctu == vbPos), 0, -1)
+        dn2 = np.where((Y > 0) & (Y % ctu == vbPos - 2), 1, 2)
+        keep = ~((above & (r == 3)) | (below & (r == 0)))[:, None]
+        for c in range(4):
+            X = bx - 2 + 2 * c
+            a, b = 2 * p(Y, X), 2 * p(Y + 1, X + 1)
+            S[0] += keep * (abs(a - p(Y + up, X) - p(Y + 1, X)) + abs(b - p(Y, X + 1) - p(Y + dn2, X + 1)))
+            S[1] += keep * (abs(a - p(Y, X + 1) - p(Y, X - 1)) + abs(b - p(Y + 1, X + 2) - p(Y + 1, X)))
+            S[2] += keep * (abs(a - p(Y + up, X - 1) - p(Y + 1, X + 1)) + abs(b - p(Y, X) - p(Y + dn2, X + 2)))
+            S[3] += keep * (abs(a - p(Y + 1, X - 1) - p(Y + up, X + 1)) + abs(b - p(Y + dn2, X) - p(Y, X + 2)))
+    sV, sH, sD0, sD1 = S
+    vb = np.broadcast_to((above | below)[:, None], sV.shape)
+    act = np.clip(((sV + sH) * np.where(vb, 96, 64)) >> (bd + 4), 0, 15)
+    hvgt, dgt = sV > sH, sD0 > sD1
+    hv1, hv0, dirHV = np.where(hvgt, sV, sH), np.where(hvgt, sH, sV), np.where(hvgt, 1, 3)
+    d1, d0, dirD = np.where(dgt, sD0, sD1), np.where(dgt, sD1, sD0), np.where(dgt, 0, 2)
+    useD = d1 * hv0 > hv1 * d0
+    hvd1, hvd0 = np.where(useD, d1, hv1), np.where(useD, d0, hv0)
+    main, sec = np.where(useD, dirD, dirHV), np.where(useD, dirHV, dirD)
+    strength = np.where(2 * hvd1 > 9 * hvd0, 2, np.where(hvd1 > 2 * hvd0, 1, 0))
+    cls = np.array([0, 1, 2, 2, 2, 2, 2, 3, 3, 3, 3, 3, 3, 3, 3, 4])[act] + np.where(strength > 0, ((main & 1) * 2 + strength) * 5, 0)
+    tr = np.array([0, 1, 0, 2, 2, 3, 1, 3])[main * 2 + (sec >> 1)]
+    cmp = np.sign(np.stack([sV - sH, sD0 - sD1, d1 * hv0 - hv1 * d0, hvd1 - 2 * hvd0, 2 * hvd1 - 9 * hvd0]))
+    nz = np.stack([sV > 0, sD0 > 0, d1 * hv0 > 0, hvd1 > 0, hvd1 > 0])
+    return dict(sV=sV, sH=sH, sD0=sD0, sD1=sD1, act=act, cls=cls, tr=tr, vb=vb, cmp=cmp, nz=nz)
+
+
+def alf_class_keys(cs, mask=None):
+    """The coverage keys of classified blocks (alf_class_sums): ('ct', class, transpose), ('act', a), ('cmp', k, sign) (sign 0 only with nonzero sides)
+    and ('vb', act > 0) for the blocks at the virtual boundary rows."""
+    m = np.ones(cs["cls"].shape, bool) if mask is None else mask
+    keys = {("ct", int(c), int(t)) for c, t in zip(cs["cls"][m], cs["tr"][m])} | {("act", int(a)) for a in np.unique(cs["act"][m])}
+    for k in range(5):
+        s, z = cs["cmp"][k][m], cs["nz"][k][m]
+        keys |= {("cmp", k, int(v)) for v in np.unique(s[(s != 0) | z])}
+    keys |= {("vb", bool(a > 0)) for a in np.unique(cs["act"][m & cs["vb"]])}
+    return keys
+
+
+def _alf_cell_pool(bd, n, seed):
+    """n 12x12 cells of mixed stripe / diagonal / checkerboard texture at amplitudes from pmax/2 down to nothing (ties between the Laplacian sums
+    are frequent at small amplitudes), plus step cells whose neighbour differences sit at every clipping value -1, +0, +1."""
+    rng = np.random.default_rng(seed)
+    pmax = (1 << bd) - 1
+    yy, xx = np.mgrid[0:12, 0:12]
+    pats = np.stack([(-1.0) ** yy, (-1.0) ** xx, np.where((xx + yy) % 4 < 2, 1.0, -1.0), np.where((xx - yy) % 4 < 2, 1.0, -1.0),
+                     np.where(yy % 4 < 2, 1.0, -1.0), np.where(xx % 4 < 2, 1.0, -1.0)])
+    wt = rng.random((n, 6)) ** rng.choice([1.0, 4.0, 12.0], size=(n, 1)) * (rng.random((n, 6)) < 0.7)
+    amp = (pmax / 2) * 2.0 ** -rng.uniform(0, bd + 1, size=(n, 1, 1))
+    cells = pmax / 2 + amp * np.tensordot(wt, pats, 1) + rng.integers(-1, 2, size=(n, 12, 12)) * rng.integers(0, 3, size=(n, 1, 1))
+    steps = []
+    for cv in alf_clip_values(bd):
+        for d in (cv - 1, cv, cv + 1):
+            d = min(d, pmax)
+            for orient in range(2):
+                s = np.where((xx if orient else yy) % 6 < 3, 0, d)
+                steps += [s, pmax - s]
+    return np.clip(np.rint(np.concatenate([cells, np.array(steps, float)])), 0, pmax).astype(np.int16)
+
+
+def _mosaic(cells, rows, cols):
+    m = np.zeros((rows * 12, cols * 12), np.int16)
+    for i in range(rows * cols):
+        r, c = divmod(i, cols)
+        m[12 * r:12 * r + 12, 12 * c:12 * c + 12] = cells[i % len(cells)]
+    return m
+
+
+_alf_select_cache = {}
+
+
+def _alf_select_cells(bd, seed=7, n=24000):
+    """Pool cells whose centre 4x4 block (classified on the cell alone) adds a coverage key not seen before, in pool order."""
+    if bd in _alf_select_cache: return _alf_select_cache[bd]
+    pool = _alf_cell_pool(bd, n, seed)
+    cols = 100
+    rows = (len(pool) + cols - 1) // cols
+    cs = alf_class_sums(_mosaic(pool, rows, cols), bd, 1 << 20)
+    i = np.arange(len(pool))
+    r, c = 3 * (i // cols) + 1, 3 * (i % cols) + 1
+    cls, tr, act, cmp, nz = cs["cls"][r, c], cs["tr"][r, c], cs["act"][r, c], cs["cmp"][:, r, c], cs["nz"][:, r, c]
+    seen, pick = set(), []
+    for k in range(len(pool)):
+        keys = {("ct", int(cls[k]), int(tr[k])), ("act", int(act[k]))} | {("cmp", j, int(cmp[j, k])) for j in range(5) if cmp[j, k] or nz[j, k]}
+        if keys - seen: seen |= keys; pick.append(k)
+    _alf_select_cache[bd] = (pool, pool[pick])
+    return _alf_select_cache[bd]
+
+
+def _alf_luma_content(kind, bd, ctu, W, H, rng):
+    pmax = (1 << bd) - 1
+    rows, cols = (H + 11) // 12, (W + 11) // 12
+    pool, chosen = _alf_select_cells(bd)
+    cells = [pool[int(i)] for i in rng.integers(0, len(pool), size=rows * cols)]
+    if kind == "classes":                                   # the chosen cells where no virtual boundary row touches their windows
+        slots = [(r, c) for r in range(rows) for c in range(cols) if 12 * r + 12 <= H and 12 * c + 12 <= W
+                 and all(not (ctu - 12 <= y % ctu < ctu + 4) and y % ctu >= 4 for y in range(12 * r, 12 * r + 12))]
+        assert len(slots) >= len(chosen), (len(slots), len(chosen))
+        for k, (r, c) in enumerate(slots[:len(chosen)]): cells[r * cols + c] = chosen[k]
+    elif kind in ("coeffs", "cc"):                          # 0 / pmax checkerboards (output and correction clips) between the texture cells
+        yy, xx = np.mgrid[0:12, 0:12]
+        board = np.where((xx + yy) % 2, pmax, 0).astype(np.int16)
+        for i in range(0, len(cells), 3 if kind == "cc" else 5): cells[i] = board if (i // 5) % 2 else pmax - board
+    return _mosaic(cells, rows, cols)[:H, :W]
+
+
+def _alf_tables(bd, part, rng):
+    """24 luma sets: the 16 fixed ones, then APS sets with +128 on every tap, one +128 per class (on tap class % 12), -128 / 127, all zero, the
+    full int8 range, the range with +128, small, and a mix; clip indices rotating over taps and classes.  8 chroma alternatives with +-128 taps.
+    4 CC-ALF filters per component whose 56 taps take the next 56 values of 0, 1, -1, ..., 64, -64 (part 0, 1, 2)."""
+    clipv = alf_clip_values(bd)
+    coef = np.zeros((24, 4, 25, 13), np.int16); clip = np.zeros((24, 4, 25, 13), np.int16)
+    coef[:16] = _fixed_sets(); clip[:16] = clipv[0]
+    k, t = np.arange(25)[:, None], np.arange(13)[None, :]
+    one = rng.integers(-20, 21, size=(25, 13)); one[np.arange(25), np.arange(25) % 12] = 128
+    mix = rng.integers(-128, 128, size=(25, 13)); mix[20:, 11] = 128
+    bases = [np.full((25, 13), 128), one, np.where((k + t) % 2, 127, -128), np.zeros((25, 13), int), rng.integers(-128, 128, size=(25, 13)),
+             rng.integers(-128, 129, size=(25, 13)), rng.integers(-8, 9, size=(25, 13)), mix]
+    for s, base in enumerate(bases, 16):
+        base = np.array(base); base[:, 12] = 128
+        bclip = np.array(clipv)[(k + t + s) % 4]
+        for tr in range(4):
+            coef[s, tr] = base[:, ALF_TR[tr]]; clip[s, tr] = bclip[:, ALF_TR[tr]]
+    a = np.arange(8)[:, None]; tt = np.arange(7)[None, :]
+    cco = np.concatenate([np.full((1, 7), 128), np.full((1, 7), -128), np.where(tt % 2, 128, -128), np.zeros((1, 7), int),
+                          rng.integers(-128, 129, size=(4, 7))]).astype(np.int16)
+    cco[:, 6] = 128
+    ccl = np.array(clipv)[(a + tt) % 4].astype(np.int16)
+    vals = [0] + [v for m in range(1, 65) for v in (m, -m)]
+    vals = (vals + [64, -64] * 30)[56 * part:56 * part + 56]
+    cc = [np.array(vals[28 * c:28 * c + 28], np.int16).reshape(4, 7) for c in range(2)]
+    return dict(lumaCoeff=np.ascontiguousarray(coef), lumaClip=np.ascontiguousarray(clip), chromaCoeff=cco, chromaClip=ccl, cc=cc)
+
+
+def _alf_records(kind, ctusW, ctusH, sets):
+    n = ctusW * ctusH
+    i = np.arange(n)
+    a = np.zeros(n, ALFCTU_DTYPE)
+    a["enable"][:, 0] = i % 5 != 4                         # unfiltered CTUs next to filtered ones
+    a["enable"][:, 1] = i % 3 != 2; a["enable"][:, 2] = i % 4 != 1
+    a["lumaSet"] = np.array(sets)[i % len(sets)]
+    a["chromaAlt"][:, 0] = i % 8; a["chromaAlt"][:, 1] = (i + 3) % 8
+    a["ccIdx"][:, 0] = i % 5; a["ccIdx"][:, 1] = (i + 2) % 5
+    if kind == "flags":                                     # every CLIP combination, corner padding and the wide chroma form where legal
+        a["enable"][:, 0] = 1 | ((i % 16) << 1)
+        cx, cy, f = i % ctusW, i // ctusW, (i % 16) << 1
+        tl = (i % 3 == 0) & (f & (ALF_CLIP_TOP_ | ALF_CLIP_LEFT_) == 0) & (cx > 0) & (cy > 0)
+        br = (i % 3 == 1) & (f & (ALF_CLIP_BOTTOM_ | ALF_CLIP_RIGHT_) == 0) & (cx < ctusW - 1) & (cy < ctusH - 1)
+        a["enable"][:, 0] |= (tl * 32 + br * 64).astype(np.uint8)
+        for c in range(2):
+            wide = (a["ccIdx"][:, c] == 0) & (i % 2 == c)
+            a["enable"][:, 1 + c] |= (wide * 2).astype(np.uint8)
+    return a
+
+
+ALF_CLIP_TOP_, ALF_CLIP_BOTTOM_, ALF_CLIP_LEFT_, ALF_CLIP_RIGHT_ = 2, 4, 8, 16
+
+# name: (kind, bit depth, CTU, W, H, chroma, strides, CC-ALF coefficient part)
+ALF_SWEEP_CASES = {
+    "classes_8bit_ctu64": ("classes", 8, 64, 384, 256, True, None, 0),
+    "classes_9bit_ctu128_last120": ("classes", 9, 128, 392, 376, True, None, 1),
+    "classes_10bit_ctu128": ("classes", 10, 128, 384, 384, True, None, 2),
+    "coeffs_10bit_ctu32_last24": ("coeffs", 10, 32, 264, 248, True, None, 0),
+    "coeffs_8bit_ctu32": ("coeffs", 8, 32, 256, 256, True, None, 1),
+    "ccalf_8bit_ctu128": ("cc", 8, 128, 264, 256, True, None, 0),
+    "ccalf_9bit_ctu64": ("cc", 9, 64, 264, 192, True, None, 1),
+    "ccalf_10bit_ctu32": ("cc", 10, 32, 264, 160, True, None, 2),
+    "flags_10bit_ctu64": ("flags", 10, 64, 520, 320, True, None, 0),
+    "flags_8bit_ctu32": ("flags", 8, 32, 264, 248, True, None, 1),
+    "geometry_400_ctu64": ("classes", 10, 64, 256, 128, False, None, 0),
+    "geometry_strides_ctu32": ("coeffs", 10, 32, 200, 136, True, (216, 108, 112), 2),
+    "uhd_3840x2160": ("mix", 10, 128, 3840, 2160, True, None, 0),
+}
+
+
+def _alf_case(name):
+    kind, bd, ctu, W, H, chroma, strides, part = ALF_SWEEP_CASES[name]
+    rng = np.random.default_rng(sum(map(ord, name)))
+    pmax = (1 << bd) - 1
+    luma = _alf_luma_content(kind, bd, ctu, W, H, rng)
+
+    def content(c, w, h):
+        if c == 0: return luma
+        if kind == "cc":                                    # chroma at 0 / pmax / mid, so the corrected sample clips both ways
+            return np.array([0, pmax, pmax // 2], np.int16)[rng.integers(0, 3, size=(h // 2 + 1, w // 2 + 1))].repeat(2, 0).repeat(2, 1)[:h, :w]
+        pool = _alf_cell_pool(bd, 400, 100 + c)
+        return _mosaic([pool[int(i)] for i in rng.integers(0, len(pool), size=((h + 11) // 12) * ((w + 11) // 12))], (h + 11) // 12, (w + 11) // 12)[:h, :w]
+    planes = _k45_planes(W, H, chroma, strides, content)
+    t = _alf_tables(bd, part, rng)
+    ctusW, ctusH = (W + ctu - 1) // ctu, (H + ctu - 1) // ctu
+    sets = list(range(24)) if kind in ("classes", "mix") else list(range(16, 24)) + [0, 15]
+    t["ctus"] = _alf_records(kind, ctusW, ctusH, sets)
+    if kind == "classes" and ctusW * ctusH < 24:            # every set on some CTU: fewer CTUs than sets in the small pictures, so rotate per case
+        t["ctus"]["lumaSet"] = (np.arange(ctusW * ctusH) * 5 + part * 7) % 24
+    g = abi.make_geom(W, H, bd, chroma_format=1 if chroma else 0, ctu=ctu, strides=strides)
+    return dict(name=name, kind=kind, g=g, W=W, H=H, bd=bd, ctu=ctu, chroma=chroma, strides=strides, planes=planes, tables=t,
+                flagged=bool((t["ctus"]["enable"][:, 0] & 0xfe).any() or (t["ctus"]["enable"][:, 1:] & 2).any()))
+
+
+def _sao_content(kind, bd, w, h, rng):
+    pmax = (1 << bd) - 1
+    if kind == "bo":                                        # every band's first, second, middle and last value, and 0 / pmax
+        bw = 1 << (bd - 5)
+        vals = np.unique([0, pmax] + [v for k in range(32) for v in (k * bw, k * bw + 1, k * bw + bw // 2, (k + 1) * bw - 1)])
+        return vals[rng.integers(0, len(vals), size=(h, w))]
+    # three levels around a base that changes every 4x4 unit (low, high, middle): plateaus (sign 0), local extremes next to 0 and pmax
+    base = np.array([0, pmax - 2, pmax // 2])[rng.integers(0, 3, size=(h // 4 + 1, w // 4 + 1))].repeat(4, 0).repeat(4, 1)[:h, :w]
+    return base + rng.integers(0, 3, size=(h, w))
+
+
+def _sao_records(kind, ctusW, ctusH, bd, chroma):
+    n = ctusW * ctusH
+    M = sao_max_offset(bd)
+    s = np.zeros(n, SAO_DTYPE)
+    s["type"] = 255
+    s["avail"] = picture_avail(ctusW, ctusH)
+    eo = [[M, M, 0, -M, -M], [1, M, 0, -M, -1], [M, 1, 0, -1, -M]]
+    for i in range(n):
+        for c in range(3 if chroma else 1):
+            if kind == "bo" or (kind == "mix" and (i + c) % 4 == 0):
+                sg = 1 if (i + c) % 2 else -1
+                s["type"][i, c] = 4; s["band"][i, c] = (i + 11 * c) % 32; s["offset"][i, c, :4] = [sg * M, -sg * M, sg * M, -sg * M]
+            elif kind == "mix" and (i + c) % 5 == 1:
+                continue
+            else:
+                s["type"][i, c] = ((i // 256 if kind == "masks" else i) + c) % 4; s["offset"][i, c] = eo[(i + c) % 3]
+    if kind == "masks":                                     # interior CTUs: every avail mask with every luma class
+        cx, cy = np.arange(n) % ctusW, np.arange(n) // ctusW
+        inner = np.flatnonzero((cx > 0) & (cx < ctusW - 1) & (cy > 0) & (cy < ctusH - 1))
+        for k, i in enumerate(inner):
+            s["avail"][i] = k % 256; s["type"][i, 0] = (k // 256) % 4
+    return s
+
+
+# name: (kind, bit depth, CTU, W, H, chroma, strides, (vertical VBs, horizontal VBs))
+SAO_SWEEP_CASES = {
+    "bo_8bit_ctu32": ("bo", 8, 32, 256, 128, True, None, ((), ())),
+    "bo_9bit_ctu32": ("bo", 9, 32, 256, 128, True, None, ((), ())),
+    "bo_10bit_ctu64": ("bo", 10, 64, 512, 256, True, None, ((), ())),
+    "bo_12bit_ctu128": ("bo", 12, 128, 1024, 512, True, None, ((), ())),
+    "eo_8bit_ctu32_partial": ("eo", 8, 32, 200, 136, True, None, ((), ())),
+    "eo_10bit_ctu64_strides": ("eo", 10, 64, 424, 240, True, (440, 216, 220), ((), ())),
+    "eo_12bit_ctu128": ("eo", 12, 128, 392, 264, True, None, ((), ())),
+    "avail_masks_ctu32": ("masks", 10, 32, 1080, 1088, True, None, ((), ())),
+    "vb_3x3_edges": ("eo", 10, 64, 384, 256, True, None, ((8, 128, 376), (8, 64, 248))),
+    "vb_3x2_mod16": ("eo", 10, 32, 320, 192, True, None, ((24, 152, 296), (40, 88))),
+    "vb_1x0_8bit": ("eo", 8, 128, 256, 128, True, None, ((136,), ())),
+    "vb_0x2_12bit": ("eo", 12, 64, 256, 192, True, None, ((), (64, 184))),
+    "vb_2x1_mix": ("mix", 10, 128, 512, 256, True, None, ((128, 264), (120,))),
+    "geometry_400": ("mix", 10, 64, 256, 128, False, None, ((), ())),
+    "geometry_400_stride": ("mix", 8, 32, 256, 128, False, (268, 0, 0), ((), ())),
+    "uhd_3840x2160": ("mix", 10, 128, 3840, 2160, True, None, ((), ())),
+}
+
+
+def _sao_case(name):
+    kind, bd, ctu, W, H, chroma, strides, (vx, vy) = SAO_SWEEP_CASES[name]
+    rng = np.random.default_rng(sum(map(ord, name)))
+    planes = _k45_planes(W, H, chroma, strides, lambda c, w, h: _sao_content("bo" if kind == "bo" else "eo", bd, w, h, rng))
+    ctusW, ctusH = (W + ctu - 1) // ctu, (H + ctu - 1) // ctu
+    vb = abi.Vb()
+    vb.numVer, vb.numHor = len(vx), len(vy)
+    for k, x in enumerate(vx): vb.posX[k] = x
+    for k, y in enumerate(vy): vb.posY[k] = y
+    g = abi.make_geom(W, H, bd, chroma_format=1 if chroma else 0, ctu=ctu, strides=strides)
+    return dict(name=name, kind=kind, g=g, W=W, H=H, bd=bd, ctu=ctu, chroma=chroma, strides=strides, planes=planes,
+                ctus=_sao_records(kind, ctusW, ctusH, bd, chroma), vb=vb)
+
+
+_k45_cache = {}
+
+
+def sao_sweep(name):
+    """One case of the designed K4 sweep (SAO_SWEEP_CASES): geometry (g, W, H, bd, ctu, chroma, strides), planes (stride padding holds -7), the CTU
+    records and the virtual boundaries (abi.Vb).  bo: every band start 0..31 with samples on every band's edges, the largest legal offsets, 0 / pmax;
+    eo: the four classes with plateaus and local extremes next to 0 / pmax, partial CTUs; masks: every avail mask with every luma class on interior
+    CTUs; vb: 0..3 vertical and horizontal boundaries at 8, W - 8, on CTU edges and at 8 mod 16."""
+    key = ("sao", name)
+    if key not in _k45_cache: _k45_cache[key] = _sao_case(name)
+    c = _k45_cache[key]
+    return dict(c, planes=[p.copy() for p in c["planes"]], ctus=c["ctus"].copy())
+
+
+def alf_sweep(name):
+    """One case of the designed K5 sweep (ALF_SWEEP_CASES): geometry, planes (stride padding holds -7) and tables (synth.gen_alf's layout, ctus
+    included).  classes: cells chosen to reach every class x transpose, activity and comparison side; coeffs: the scalar-path and int8-extreme APS
+    sets on 0 / pmax checkerboards and clip steps; cc: every CC-ALF coefficient value over 0 / pmax luma and chroma; flags: every CLIP combination,
+    PAD_TL / PAD_BR and PAD_WIDE.  flagged: whether any CTU has clip / pad flags."""
+    key = ("alf", name)
+    if key not in _k45_cache: _k45_cache[key] = _alf_case(name)
+    c = _k45_cache[key]
+    t = c["tables"]
+    return dict(c, planes=[p.copy() for p in c["planes"]], tables=dict(t, ctus=t["ctus"].copy(), cc=[x.copy() for x in t["cc"]]))
+
+
+# ---- the record rules of b200_sao_picture / b200_alf_picture (vvdec_b200/csrc/api.cu), for the CPU tests
+def k45_geom_problems(g, max_bd):
+    out = []
+    if g.chromaFormat not in (0, 1): out.append(f"chromaFormat {g.chromaFormat}")
+    if g.ctuSize not in (32, 64, 128): out.append(f"CTU size {g.ctuSize}")
+    if not 8 <= g.bitDepth <= max_bd: out.append(f"bit depth {g.bitDepth}")
+    if g.width <= 0 or g.height <= 0 or g.width % 8 or g.height % 8: out.append(f"picture {g.width}x{g.height}")
+    for c in range(3 if g.chromaFormat else 1):
+        pw = g.width >> (c > 0)
+        if g.stride[c] < pw or g.stride[c] % 4: out.append(f"plane {c} stride {g.stride[c]}")
+    return out
+
+
+def k45_record_problems(kind, g, ctus, tables=None, vb=None):
+    """What b200_sao_picture (kind 'sao') / b200_alf_picture ('alf') refuses in a geometry, its CTU records and tables or virtual boundaries: a list of
+    reasons, empty for a call it accepts."""
+    out = k45_geom_problems(g, 12 if kind == "sao" else 10)
+    if out: return out                                      # the records are not read for a geometry that is refused
+    ctusW, ctusH = (g.width + g.ctuSize - 1) // g.ctuSize, (g.height + g.ctuSize - 1) // g.ctuSize
+    n = ctusW * ctusH
+    if kind == "sao":
+        nc = 3 if g.chromaFormat else 1
+        for i in range(n):
+            for c in range(nc):
+                t = int(ctus["type"][i, c])
+                if t != 255 and t > 4: out.append(f"CTU {i} type {t}")
+                if t == 4 and ctus["band"][i, c] > 31: out.append(f"CTU {i} band {ctus['band'][i, c]}")
+        if vb is not None:
+            if not (0 <= vb.numVer <= 3 and 0 <= vb.numHor <= 3): out.append("virtual boundary count")
+            else:
+                out += [f"vertical VB {vb.posX[k]}" for k in range(vb.numVer) if not (0 < vb.posX[k] < g.width and vb.posX[k] % 8 == 0)]
+                out += [f"horizontal VB {vb.posY[k]}" for k in range(vb.numHor) if not (0 < vb.posY[k] < g.height and vb.posY[k] % 8 == 0)]
+        return out
+    T = tables
+    nL, nC, nCc = T["lumaCoeff"].shape[0], T["chromaCoeff"].shape[0], [T["cc"][c].shape[0] for c in range(2)]
+    if not 16 <= nL <= 24: out.append(f"numLumaSets {nL}")
+    if nC < 0: out.append(f"numChromaAlts {nC}")
+    out += [f"numCc[{c}] {nCc[c]}" for c in range(2) if nCc[c] < 0]
+    for i in range(n):
+        a = ctus[i]
+        f, cx, cy = int(a["enable"][0]), i % ctusW, i // ctusW
+        if f & 0x80 or int(a["enable"][1]) & ~3 or int(a["enable"][2]) & ~3: out.append(f"CTU {i} enable bits")
+        if f & 1 and a["lumaSet"] >= nL: out.append(f"CTU {i} lumaSet {a['lumaSet']}")
+        for c in range(2):
+            if a["enable"][1 + c] & 1 and a["chromaAlt"][c] >= nC: out.append(f"CTU {i} chromaAlt[{c}] {a['chromaAlt'][c]}")
+            if a["ccIdx"][c] > nCc[c]: out.append(f"CTU {i} ccIdx[{c}] {a['ccIdx'][c]}")
+            if a["enable"][1 + c] & 2 and a["ccIdx"][c]: out.append(f"CTU {i} PAD_WIDE with CC-ALF")
+        if f & 32 and (f & (ALF_CLIP_TOP_ | ALF_CLIP_LEFT_) or cx == 0 or cy == 0): out.append(f"CTU {i} PAD_TL")
+        if f & 64 and (f & (ALF_CLIP_BOTTOM_ | ALF_CLIP_RIGHT_) or cx == ctusW - 1 or cy == ctusH - 1): out.append(f"CTU {i} PAD_BR")
+    return out
