@@ -89,7 +89,9 @@ def test_k1_isp_thin_partitions(b200, oracle):
     planes = synth.noise_planes(rng, W, H, 10)
     for field, val in (("comp", 1), ("lfnst", 1)):
         bad = tus[:1].copy(); bad[field] = val
-        assert b200.b200_k1_residual(C.byref(g), abi.plane_ptrs(planes), bad.ctypes.data, 1, arena.ctypes.data, len(arena), None, 0, 0) != 0
+        got = [p.copy() for p in planes]
+        assert b200.b200_k1_residual(C.byref(g), abi.plane_ptrs(got), bad.ctypes.data, 1, arena.ctypes.data, len(arena), None, 0, 0) == -2, field
+        assert b"TU record 0" in b200.b200_last_error() and all(np.array_equal(a, b) for a, b in zip(got, planes)), field
 
 
 def test_k1_empty_and_errors(b200):

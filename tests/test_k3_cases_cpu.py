@@ -1,7 +1,7 @@
 """The designed K3 sweep (synth.lf_sweep) on the CPU: its grids are legal for the flat pass, every designed segment takes the decision it was built
 for with its thresholds where they were put, the oracle changes only samples the classified decisions may write, and the sweep as a whole covers
-every decision with every threshold on both sides.  Also: the grid rule (synth.lf_grid_problems) accepts the golden grids and gen_lf_grid's, and
-refuses each row of the refusal table that b200_lf_deblock refuses (tests/test_k3_gpu.py)."""
+every decision with every threshold on both sides.  Also: b200_lf_deblock, asked through synth.lf_grid_problems / lf_problems (its checks all run on the
+host), accepts the golden grids and gen_lf_grid's, and refuses each row of the refusal table (tests/test_k3_gpu.py runs the accepted calls)."""
 import os
 import numpy as np
 import pytest
@@ -162,7 +162,7 @@ def _cs(i, v):
     return f
 
 
-# (what, edit that breaks a rule, the same edit with the offending field fixed, whether the Python grid rule sees it)
+# (what, edit that breaks a rule, the same edit with the offending field fixed, whether it breaks a rule of the grid scan)
 REFUSALS = [
     ("chromaFormat 2", _geom(chromaFormat=2), _geom(chromaFormat=1), False), ("chromaFormat 3", _geom(chromaFormat=3), _geom(chromaFormat=0), False),
     ("bit depth 7", _geom(bitDepth=7), _geom(bitDepth=8), False), ("bit depth 13", _geom(bitDepth=13), _geom(bitDepth=12), False),
@@ -194,11 +194,14 @@ def refusal_variant(edit):
     return k
 
 
-@pytest.mark.parametrize("what,bad,fixed,grid", [r for r in REFUSALS if r[3]], ids=[r[0] for r in REFUSALS if r[3]])
+@pytest.mark.parametrize("what,bad,fixed,grid", REFUSALS, ids=[r[0] for r in REFUSALS])
 def test_rule_rows(what, bad, fixed, grid):
-    """The grid rows of the refusal table: the Python rule refuses each edit and accepts it with the offending field fixed."""
-    base = refusal_base()
-    assert all(synth.lf_grid_legal(base["lfH" if d else "lfV"], d, base["g"]) for d in (0, 1))
-    for edit, legal in ((bad, False), (fixed, True)):
-        k = refusal_variant(edit)
-        assert all(synth.lf_grid_legal(k["lfH" if d else "lfV"], d, k["g"]) for d in (0, 1)) == legal, (what, legal)
+    """Every row of the refusal table: b200_lf_deblock refuses the edit, naming itself, and accepts it with the offending field fixed; a grid row is
+    refused for its grid alone."""
+    assert synth.lf_problems(refusal_base()) == []
+    probs = synth.lf_problems(refusal_variant(bad))
+    assert len(probs) == 1 and "b200_lf_deblock" in probs[0], (what, probs)
+    assert synth.lf_problems(refusal_variant(fixed)) == [], what
+    if grid:
+        k = refusal_variant(bad)
+        assert not all(synth.lf_grid_legal(k["lfH" if d else "lfV"], d, k["g"]) for d in (0, 1)), what

@@ -1,8 +1,8 @@
 """The designed K4 / K5 sweep (synth.sao_sweep, synth.alf_sweep) on the CPU: the classification restatement (synth.alf_class_sums) equals the oracle's
 on every block, the sweep reaches every ALF class x transpose, activity and comparison side, every SAO category x class, every avail mask with every
-class, every band start with samples in and just outside its four bands, and the clips of both filters.  Also: the record rule
-(synth.k45_record_problems) accepts the generated, golden and sweep records and refuses each row of the refusal table that b200_sao_picture /
-b200_alf_picture refuse (tests/test_k45_gpu.py)."""
+class, every band start with samples in and just outside its four bands, and the clips of both filters.  Also: b200_sao_picture / b200_alf_picture,
+asked through synth.k45_record_problems (their checks all run on the host), accept the generated, golden and sweep records and refuse each row of
+the refusal table (tests/test_k45_gpu.py runs the accepted calls)."""
 import ctypes as C
 import numpy as np
 import pytest
@@ -285,10 +285,11 @@ def refusal_variant(kind, edit):
 
 @pytest.mark.parametrize("kind,what,bad,fixed", REFUSALS, ids=[f"{r[0]}: {r[1]}" for r in REFUSALS])
 def test_rule_rows(kind, what, bad, fixed):
-    """The Python rule refuses each edit and accepts it with the offending field fixed."""
+    """The library refuses each edit, naming the entry point, and accepts it with the offending field fixed."""
     base = refusal_base(kind)
     assert synth.k45_record_problems(kind, base["g"], base["ctus"], base["tables"], base["vb"]) == []
     for edit, legal in ((bad, False), (fixed, True)):
         k = refusal_variant(kind, edit)
         probs = synth.k45_record_problems(kind, k["g"], k["ctus"], k["tables"], k["vb"])
         assert (probs == []) == legal, (what, legal, probs)
+        assert legal or f"b200_{kind}_picture" in probs[0], (what, probs)

@@ -43,10 +43,45 @@ def test_gop_decompress(b200, oracle, seed, W, H, flagsets):
 
 
 def test_ctx_errors(b200):
-    g = abi.make_geom(100, 64, 10)
     ctx = C.c_void_p()
-    assert b200.b200_ctx_create(C.byref(ctx), C.byref(g), 4, 2, -1) == -2
-    assert b"multiple of 8" in b200.b200_last_error()
+    for g, what in ((abi.make_geom(100, 64, 10), b"multiple of 8"), (abi.make_geom(64, 64, 7), b"bit depth"), (abi.make_geom(64, 64, 13), b"bit depth"),
+                    (abi.make_geom(64, 64, 10, strides=(64, 32, 31)), b"stride")):
+        assert b200.b200_ctx_create(C.byref(ctx), C.byref(g), 4, 2, -1) == -2, what
+        assert what in b200.b200_last_error() and b"b200_ctx_create" in b200.b200_last_error()
+
+
+def test_pic_upload_refuses_tables_and_boundaries(b200):
+    """b200_pic_upload refuses the ALF table counts (a picture's tables may hold several slices' APS sets: up to 255 luma sets) and SAO virtual
+    boundaries b200_alf_picture / b200_sao_picture refuse, before it copies anything; the same picture with the field restored decodes."""
+    rng = np.random.default_rng(8)
+    W, H, bd = 416, 240, 10
+    g = abi.make_geom(W, H, bd)
+    ctx = C.c_void_p()
+    vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 2, -1))
+    try:
+        pic = synth.gen_picture(rng, W, H, bd, dst_slot=4)
+        T, vb = pic["alfTabs"], abi.Vb()
+        vb.numVer, vb.numHor, vb.posX[0], vb.posY[0] = 1, 1, 64, 120
+        pic["struct"].vb = C.addressof(vb)
+        def refused(what):
+            return b200.b200_pic_upload(ctx, C.byref(pic["struct"])) == -2 and what in b200.b200_last_error() and b"b200_pic_upload" in b200.b200_last_error()
+        n, cc = T.numLumaSets, T.numCc[0]
+        for bad in (15, 256):
+            T.numLumaSets = bad
+            assert refused(b"numLumaSets"), bad
+        T.numLumaSets = n
+        T.numCc[0] = -1
+        assert refused(b"numCc")
+        T.numCc[0] = cc
+        vb.posX[0] = 68
+        assert refused(b"vertical virtual boundary")
+        vb.posX[0], vb.posY[0] = 64, 244
+        assert refused(b"horizontal virtual boundary")
+        vb.posY[0] = 120
+        h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"])); assert h >= 0, b200.b200_last_error()
+        assert b200.b200_wait_picture(ctx, h, None, 0) == 0
+    finally:
+        b200.b200_ctx_destroy(ctx)
 
 
 def test_invalid_records_are_reported(b200):

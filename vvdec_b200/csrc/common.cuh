@@ -7,6 +7,7 @@
 #include <vector>
 #include <algorithm>
 #include "../../include/vvdec_b200.h"
+#include "rules.cuh"
 
 namespace b200 {
 
@@ -98,7 +99,6 @@ constexpr int K1_LISTS = 4;      // TU max dimension <= 8, 16, 32, 64
 constexpr int LM_CNT = 0, LM_OFF = 32, LM_CUR = 64, LM_DONE = 96, LM_ERR = 97, LM_INTS = 128;   // meta layout: counts, offsets, cursors, ticket, error bits
 int launch_mc_bucket(const b200_pu* pus, size_t numPus, uint32_t* tiles, size_t capTiles, int* meta, const b200_geom& g, int numSlots, int numWp, size_t numDmvr, cudaStream_t s);
 int launch_tu_bucket(const b200_tu* tus, size_t numTus, uint32_t* idx, int* meta, const b200_geom& g, size_t numCoefs, size_t numScaling, cudaStream_t s);
-struct CtuLimits { int numLumaSets, numChromaAlts, numCc[2], numLfSlices, ctusW, ctusH; };
 int launch_ctu_validate(const b200_sao_ctu* sao, const b200_alf_ctu* alf, const uint8_t* ctuSlice, int nCtu, const CtuLimits& lim, int* meta, cudaStream_t s);   // after launch_mc_bucket (same meta block)
 size_t mc_tile_capacity(const b200_geom& g, size_t numPus);
 int num_sms();                   // SM count of the current device (persistent-style grids are sized from it)
@@ -175,29 +175,6 @@ struct IntraLaunch { b200_geom geom; DevPlanes planes; const int16_t* resi[3]; c
                                                 // the chroma residual scale of a VPDU is derived from the finished luma, so luma goes first)
                    };
 inline size_t intra_order_ints(const b200_geom& g, size_t numTus) { return numTus + 8 + 3 * (size_t)((g.width + g.ctuSize - 1) / g.ctuSize) * ((g.height + g.ctuSize - 1) / g.ctuSize); }
-inline int intra_ctu_log2(const b200_geom& g) { return g.ctuSize == 128 ? 7 : g.ctuSize == 64 ? 6 : 5; }
-// the block (or ISP region) of a record lies inside one CTU (chroma: CTU size halved): the CTU-resident kernel addresses its tile by the CTU of the
-// block's top-left sample, so a block reaching into the next CTU would write outside its tile rows
-__host__ __device__ inline bool intra_record_in_ctu(const b200_intra_tu& t, int ctuLog2)
-{
-  const int cl = ctuLog2 - (t.comp ? 1 : 0);
-  return (t.x >> cl) == ((t.x + (1 << t.log2w) - 1) >> cl) && (t.y >> cl) == ((t.y + (1 << t.log2h) - 1) >> cl);
-}
-// ISP region record (B200_INTRA_ISP, include/vvdec_b200.h): everything K6 derives addresses from.  prev = the record before it in the list (null for the first).
-__host__ __device__ inline bool intra_isp_record_ok(const b200_intra_tu& t, const b200_intra_tu* prev, int W, int H)
-{
-  const int sp = t.mip & 3, k = (t.mip >> 2) & 3, l2n = (t.mip >> 4) & 3, nReg = 1 << l2n, rw = 1 << t.log2w, rh = 1 << t.log2h;
-  if (t.comp || t.mode > 66 || t.multiRefIdx || (sp != 1 && sp != 2) || l2n > 2 || (l2n == 0 && (sp != 2 || rw != 4)) /* one region: a 4-wide CU split into 1- or 2-sample columns */ || k >= nReg || (t.mip >> 6) || t.log2w < 2 || t.log2w > 6 || t.log2h > 6) return false;
-  const int cw = sp == 2 ? rw * nReg : rw, ch = sp == 1 ? rh * nReg : rh, cx = t.x - (sp == 2 ? k * rw : 0), cy = t.y - (sp == 1 ? k * rh : 0);
-  if (cw > 64 || ch > 64 || ch < 4 || cw * ch < 32 || cx < 0 || cy < 0 || (cx & 3) || (cy & 3) || cx + cw > W || cy + ch > H) return false;
-  if (t.numAbove > 2 * cw / 4 || t.numLeft > 2 * ch / 4 || (t.numAbove && !cy) || (t.numLeft && !cx) || ((t.flags & B200_INTRA_AVAIL_TL) && (!cx || !cy))
-      || cx + (int)t.numAbove * 4 > W || cy + (int)t.numLeft * 4 > H || (t.lmLeft && !cx) || (t.lmAbove && !cy)) return false;
-  if (k) {                                                     // the region before it is the record before it
-    if (!prev || !(prev->flags & B200_INTRA_ISP) || prev->mip != (uint8_t)(t.mip - 4) || prev->log2w != t.log2w || prev->log2h != t.log2h || prev->mode != t.mode
-        || prev->x != t.x - (sp == 2 ? rw : 0) || prev->y != t.y - (sp == 1 ? rh : 0)) return false;
-  }
-  return true;
-}
 int launch_intra(const IntraLaunch& L, cudaStream_t s);
 int launch_intra_ciip_clear(const b200_intra_tu* tus, size_t numTus, int16_t* const resi[3], const int stride[3], cudaStream_t s);   // before K1: see k6_intra.cu
 int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_geom& g, int* meta, cudaStream_t s);   // error bit 8 of the PU meta block (after launch_mc_bucket)

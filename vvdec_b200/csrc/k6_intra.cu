@@ -914,24 +914,14 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
   }
 }
 
-// record checks of the picture path (the kernel-level wrapper checks on the host): everything K6 uses as an address
-__global__ void __launch_bounds__(256) intra_validate_kernel(const b200_intra_tu* __restrict__ tus, int n, int W, int H, int chroma, int ctuLog2, int* meta)
+// record checks of the picture path (the kernel-level wrapper checks on the host)
+__global__ void __launch_bounds__(256) intra_validate_kernel(const b200_intra_tu* __restrict__ tus, int n, const b200_geom g, int* meta)
 {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= n) return;
-  const b200_intra_tu t = tus[i];
-  if (!intra_record_in_ctu(t, ctuLog2)) { atomicOr(&meta[LM_ERR], 8); return; }
-  if (t.flags & B200_INTRA_ISP) { b200_intra_tu prev; if (i) prev = tus[i - 1]; if (!intra_isp_record_ok(t, i ? &prev : nullptr, W, H)) atomicOr(&meta[LM_ERR], 8); return; }
-  const int w = 1 << t.log2w, h = 1 << t.log2h, pw = t.comp ? W >> 1 : W, ph = t.comp ? H >> 1 : H, unit = t.comp ? 2 : 4, m = t.multiRefIdx;
-  bool ok = t.comp < (chroma ? 3 : 1) && t.log2w >= 2 && t.log2w <= 6 && t.log2h >= 1 && t.log2h <= 6 && t.x + w <= pw && t.y + h <= ph && !(t.x % unit) && !(t.y % unit);
-  ok = ok && t.mode <= B200_INTRA_MDLM_T && m <= 2 && (!m || !t.comp);
-  if (t.ciip) ok = ok && t.ciip <= 3 && t.mode == B200_INTRA_PLANAR;
-  if (t.mode >= B200_INTRA_LM) ok = ok && t.comp && t.log2w <= 5 && t.log2h <= 5 && t.lmAbove <= w && t.lmLeft <= h && (!(t.flags & B200_INTRA_LM_ABOVE) || t.y >= 2) && (!(t.flags & B200_INTRA_LM_LEFT) || t.x >= 2)
-                                  && t.x + max(w, 2 * t.lmAbove) <= pw && t.y + max(h, 2 * t.lmLeft) <= ph;
-  if (t.mode == B200_INTRA_MIP) ok = ok && !t.comp && !m && (t.mip & 0x7f) < ((w == 4 && h == 4) ? 16 : (w == 4 || h == 4 || (w == 8 && h == 8)) ? 8 : 6);
-  ok = ok && t.numAbove <= 2 * w / unit && t.numLeft <= 2 * h / unit && (!t.numAbove || t.y > m) && (!t.numLeft || t.x > m)
-          && (!(t.flags & B200_INTRA_AVAIL_TL) || (t.x > m && t.y > m)) && t.x + (int)t.numAbove * unit <= pw && t.y + (int)t.numLeft * unit <= ph;
-  if (!ok) atomicOr(&meta[LM_ERR], 8);
+  b200_intra_tu prev;
+  if (i) prev = tus[i - 1];
+  if (intra_problem(tus[i], i ? &prev : nullptr, g)) atomicOr(&meta[LM_ERR], 8);
 }
 
 #ifdef B200_K6_PROF
@@ -974,7 +964,7 @@ int launch_intra_ciip_clear(const b200_intra_tu* tus, size_t numTus, int16_t* co
 int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_geom& g, int* meta, cudaStream_t s)
 {
   if (!numTus) return 0;
-  intra_validate_kernel<<<(unsigned)((numTus + 255) / 256), 256, 0, s>>>(tus, (int)numTus, g.width, g.height, g.chromaFormat != 0, intra_ctu_log2(g), meta);
+  intra_validate_kernel<<<(unsigned)((numTus + 255) / 256), 256, 0, s>>>(tus, (int)numTus, g, meta);
   B200_CUDA(cudaGetLastError());
   return 0;
 }

@@ -80,9 +80,7 @@ B200_API int b200_ctx_create(b200_ctx** out, const b200_geom* g, int numSlots, i
 {
   B200_CHECK(out && g, "b200_ctx_create: null argument");
   B200_CHECK(numSlots >= 1 && numSlots <= B200_MAX_SLOTS && numArenas >= 1 && numArenas <= 256, "b200_ctx_create: numSlots %d / numArenas %d out of range", numSlots, numArenas);
-  B200_CHECK((g->width & 7) == 0 && (g->height & 7) == 0, "b200_ctx_create: picture size must be a multiple of 8");
-  B200_CHECK(g->chromaFormat == 0 || g->chromaFormat == 1, "b200_ctx_create: only 4:0:0 and 4:2:0");
-  B200_CHECK(g->ctuSize == 32 || g->ctuSize == 64 || g->ctuSize == 128, "b200_ctx_create: CTU size %d", g->ctuSize);
+  if (const char* why = geom_problem(*g, 12, 1)) { set_error("b200_ctx_create: %s", why); return B200_ERR_PARAM; }
   if (int rc = ensure_device()) return rc;
   if (device >= 0) B200_CUDA(cudaSetDevice(device));
   b200_ctx* c = new b200_ctx;
@@ -150,11 +148,13 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   B200_CHECK(p->dstSlot >= 0 && p->dstSlot < c->numSlots, "b200_pic_upload: dstSlot %d", p->dstSlot);
   B200_CHECK(!(p->flags & B200_PIC_DEBLOCK) || (p->lfV && p->lfH && p->lfSlices && p->numLfSlices >= 1 && p->numLfSlices <= 64), "b200_pic_upload: deblocking data missing");
   B200_CHECK(!(p->flags & B200_PIC_SAO) || p->sao, "b200_pic_upload: SAO data missing");
-  B200_CHECK(!(p->flags & B200_PIC_ALF) || (p->alf && p->alfTabs && p->alfTabs->numLumaSets >= 16), "b200_pic_upload: ALF data missing");
-  B200_CHECK(!(p->flags & B200_PIC_ALF) || c->g.bitDepth <= 10, "b200_pic_upload: ALF at bit depth %d (ALF is defined up to 10 bit)", c->g.bitDepth);
-  // K4 and K5 move 4 samples per 8-byte access on every plane
-  B200_CHECK(!(p->flags & (B200_PIC_SAO | B200_PIC_ALF)) || (!(c->g.stride[0] & 3) && (!c->g.chromaFormat || (!(c->g.stride[1] & 3) && !(c->g.stride[2] & 3)))),
-             "b200_pic_upload: SAO / ALF need every plane stride to be a multiple of 4 (strides %d, %d, %d)", c->g.stride[0], c->g.stride[1], c->g.stride[2]);
+  B200_CHECK(!(p->flags & B200_PIC_ALF) || (p->alf && p->alfTabs), "b200_pic_upload: ALF data missing");
+  // the O(1) rules of b200_sao_picture / b200_alf_picture (rules.cuh); the CTU records are checked on the device
+  const char* why = nullptr;
+  if (p->flags & (B200_PIC_SAO | B200_PIC_ALF)) why = geom_problem(c->g, (p->flags & B200_PIC_ALF) ? 10 : 12, 4);
+  if (!why && (p->flags & B200_PIC_ALF)) why = alf_tables_problem(*p->alfTabs, 255);   // a picture's tables hold every slice's APS sets
+  if (!why && (p->flags & B200_PIC_SAO) && p->vb) why = vb_problem(*p->vb, c->g.width, c->g.height);
+  if (why) { set_error("b200_pic_upload: %s", why); return B200_ERR_PARAM; }
   B200_CHECK(p->numPus < (1u << 26) && p->numTus < (1u << 31), "b200_pic_upload: too many records");
   B200_CHECK(p->numWp >= 0 && p->numWp <= 255 && (p->wp || !p->numWp), "b200_pic_upload: weighted-prediction table (at most 255 entries)");
   B200_CHECK(!(p->flags & B200_PIC_LMCS) || (p->lmcs && p->lmcs->invLUT && (!p->lmcs->chromaAdj || p->lmcs->vpdus) && p->lmcs->orgCW == (1 << c->g.bitDepth) / 16), "b200_pic_upload: LMCS data missing or inconsistent");
@@ -261,12 +261,9 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   A.tiles = reinterpret_cast<const uint32_t*>(base + oT); A.tuIdx = reinterpret_cast<const uint32_t*>(base + oIdx);
   c->launches += 4;
   {
-    CtuLimits lim; const bool alfOn = p->flags & B200_PIC_ALF;
-    lim.numLumaSets = alfOn ? T->numLumaSets : 0; lim.numChromaAlts = alfOn ? T->numChromaAlts : 0; lim.numCc[0] = alfOn ? T->numCc[0] : 0; lim.numCc[1] = alfOn ? T->numCc[1] : 0;
-    lim.numLfSlices = p->numLfSlices;
-    lim.ctusW = (g.width + g.ctuSize - 1) / g.ctuSize; lim.ctusH = (g.height + g.ctuSize - 1) / g.ctuSize;
-    const bool any = (p->flags & (B200_PIC_SAO | B200_PIC_ALF)) || ((p->flags & B200_PIC_DEBLOCK) && p->ctuSlice);
-    if (int rc = launch_ctu_validate((p->flags & B200_PIC_SAO) ? A.sao : nullptr, alfOn ? A.alf : nullptr, (p->flags & B200_PIC_DEBLOCK) ? A.ctuSlice : nullptr, (int)nCtu, lim, A.mcMeta, s)) return rc;
+    const bool alfOn = p->flags & B200_PIC_ALF, any = (p->flags & (B200_PIC_SAO | B200_PIC_ALF)) || ((p->flags & B200_PIC_DEBLOCK) && p->ctuSlice);
+    if (int rc = launch_ctu_validate((p->flags & B200_PIC_SAO) ? A.sao : nullptr, alfOn ? A.alf : nullptr, (p->flags & B200_PIC_DEBLOCK) ? A.ctuSlice : nullptr, (int)nCtu,
+                                     ctu_limits(g, alfOn ? T : nullptr, p->numLfSlices), A.mcMeta, s)) return rc;
     if (any) c->launches += 1;
   }
   if (A.numIntraTus) { if (int rc = launch_intra_validate(A.intraTus, A.numIntraTus, g, A.mcMeta, s)) return rc; c->launches += 1; }

@@ -1,6 +1,7 @@
 """Synthetic post-parse content (SURVEY.md §8d): there is no VVC bitstream or encoder on the box, so the
 work lists a flattener would emit from VVdeC's parsed Picture are drawn from a seeded generator instead.
 Everything here is host-side input preparation (numpy); no pixel arithmetic of the hot path lives here."""
+import ctypes as C
 import numpy as np
 from . import abi
 
@@ -1454,44 +1455,6 @@ def lf_decisions(planes, grid, d, g, slices, seq=None, ctu_slice=None):
     return out
 
 
-LF_READS = {1: 3, 2: 3, 3: 4, 5: 6, 7: 8}
-
-
-def lf_grid_problems(grid, d, g, limit=8):
-    """What the flat pass of K3 needs from one direction's grid (d: 0 lfV, 1 lfH), as b200_lf_deblock checks it: the first `limit` edges that break a
-    rule, as strings (empty: legal).  Per side, a luma edge of length n writes n samples and reads LF_READS[n]; on a horizontal edge at a CTU row the P
-    side counts as 3, and when one side is long (5, 7) the other counts as at least 3 (the long filter runs it as 3).  Rules: Bs fields are 0..2; no
-    edge with Bs != 0 on the picture's first column (lfV) / row (lfH); luma lengths of an edge with luma Bs != 0 are 1, 2, 3, 5 or 7; no side reads past
-    the picture; and two luma edges at e1 < e2 on one line need e2 - e1 >= writesQ(e1) + readsP(e2) and e2 - e1 >= readsQ(e1) + writesP(e2)."""
-    out = []
-    bs = grid["bs"].astype(np.int64) & 0x3f
-    extent = g.height if d else g.width
-    lines, poss = np.nonzero(bs.T if d else bs)
-    prev = {}
-    for line, k in zip(lines.tolist(), poss.tolist()):
-        y4, x4 = (k, line) if d else (line, k)
-        e, pos, where = grid[y4, x4], 4 * k, f"{'lfH' if d else 'lfV'} ({4 * x4}, {4 * y4})"
-        b = int(e["bs"]) & 0x3f
-        if 3 in (b & 3, (b >> 2) & 3, b >> 4): out.append(f"{where}: Bs 3")
-        elif pos == 0: out.append(f"{where}: Bs != 0 on the picture's border")
-        elif b & 3:
-            nP, nQ = (int(e["len"]) >> 4) & 7, int(e["len"]) & 7
-            if nP not in LF_READS or nQ not in LF_READS: out.append(f"{where}: luma lengths {nP}/{nQ}"); continue
-            if d and pos % g.ctuSize == 0: nP = min(nP, 3)
-            wP, wQ = (max(nP, 3), max(nQ, 3)) if max(nP, nQ) > 3 else (nP, nQ)
-            rP, rQ = LF_READS[wP], LF_READS[wQ]
-            if pos < rP or pos + rQ > extent: out.append(f"{where}: lengths {nP}/{nQ} read outside the picture")
-            elif line in prev and (pos - prev[line][0] < prev[line][1] + rP or pos - prev[line][0] < prev[line][2] + wP):
-                out.append(f"{where}: {pos - prev[line][0]} samples after the previous edge")
-            prev[line] = (pos, wQ, rQ)
-        if len(out) >= limit: break
-    return out
-
-
-def lf_grid_legal(grid, d, g):
-    return not lf_grid_problems(grid, d, g, limit=1)
-
-
 def _lf_side(v, d=0, s=0, dx=0, e=0, a1=0):
     """Eight samples of one side of an edge, nearest first, around level v: |x2 - 2 x1 + x0| = d, |x3 - x0| = s, |x5 - 2 x4 + x3| = dx, and at length 7
     |x4 - x5 - x6 + x7| = e with x7 = x3 (length 5: |x3 - x5| = dx); a1 = x1 - x0 (the chroma CTB form's |p1 - p0|)."""
@@ -2152,53 +2115,49 @@ def alf_sweep(name):
     return dict(c, planes=[p.copy() for p in c["planes"]], tables=dict(t, ctus=t["ctus"].copy(), cc=[x.copy() for x in t["cc"]]))
 
 
-# ---- the record rules of b200_sao_picture / b200_alf_picture (vvdec_b200/csrc/api.cu), for the CPU tests
-def k45_geom_problems(g, max_bd):
-    out = []
-    if g.chromaFormat not in (0, 1): out.append(f"chromaFormat {g.chromaFormat}")
-    if g.ctuSize not in (32, 64, 128): out.append(f"CTU size {g.ctuSize}")
-    if not 8 <= g.bitDepth <= max_bd: out.append(f"bit depth {g.bitDepth}")
-    if g.width <= 0 or g.height <= 0 or g.width % 8 or g.height % 8: out.append(f"picture {g.width}x{g.height}")
-    for c in range(3 if g.chromaFormat else 1):
-        pw = g.width >> (c > 0)
-        if g.stride[c] < pw or g.stride[c] % 4: out.append(f"plane {c} stride {g.stride[c]}")
-    return out
+# ---- what the library refuses: its kernel-level entry points check every rule (vvdec_b200/csrc/rules.cuh) on the host, before any device work, so
+# these ask it on any machine.  Without a GPU a legal call returns B200_ERR_NO_DEVICE; on one it runs, on zero planes of the geometry.
+def library_refusal(fn, *args):
+    """The error message of the library's entry point `fn` when it refuses the call with `args` (B200_ERR_PARAM), else None."""
+    from . import lib
+    return lib().b200_last_error().decode() if getattr(lib(), fn)(*args) == -2 else None
+
+
+def _zero_planes(g):
+    return [np.zeros((g.height >> (c > 0), g.stride[c]), np.int16) if c == 0 or g.chromaFormat else None for c in range(3)]
+
+
+def lf_problems(case):
+    """What b200_lf_deblock says about a call of lf_sweep's form (g, lfV, lfH; ctuSlice, slices, seq and dirs default to none, one slice, no LADF and 3):
+    [] when it accepts the call, else [its error message]."""
+    k = dict(dict(ctuSlice=None, slices=np.zeros(1, LFSLICE_DTYPE), seq=abi.LfSeq(), dirs=3), **case)
+    lfV, lfH, cs, planes = np.ascontiguousarray(k["lfV"]), np.ascontiguousarray(k["lfH"]), k["ctuSlice"], _zero_planes(k["g"])   # alive until the call returns
+    msg = library_refusal("b200_lf_deblock", C.byref(k["g"]), abi.plane_ptrs(planes), lfV.ctypes.data, lfH.ctypes.data,
+                          None if cs is None else cs.ctypes.data, k["slices"].ctypes.data, len(k["slices"]), C.addressof(k["seq"]), k["dirs"])
+    return [] if msg is None else [msg]
+
+
+def lf_grid_problems(grid, d, g):
+    """What b200_lf_deblock says about the grid of direction d (0 lfV, 1 lfH) of geometry g, the other direction without edges."""
+    z = np.zeros_like(grid)
+    return lf_problems(dict(g=g, lfV=z if d else grid, lfH=grid if d else z))
+
+
+def lf_grid_legal(grid, d, g):
+    return not lf_grid_problems(grid, d, g)
 
 
 def k45_record_problems(kind, g, ctus, tables=None, vb=None):
-    """What b200_sao_picture (kind 'sao') / b200_alf_picture ('alf') refuses in a geometry, its CTU records and tables or virtual boundaries: a list of
-    reasons, empty for a call it accepts."""
-    out = k45_geom_problems(g, 12 if kind == "sao" else 10)
-    if out: return out                                      # the records are not read for a geometry that is refused
-    ctusW, ctusH = (g.width + g.ctuSize - 1) // g.ctuSize, (g.height + g.ctuSize - 1) // g.ctuSize
-    n = ctusW * ctusH
+    """What b200_sao_picture (kind 'sao') / b200_alf_picture ('alf') says about a geometry, its CTU records and tables (gen_alf's layout: only the
+    numbers of sets count) or virtual boundaries: [] when it accepts the call, else [its error message]."""
+    src, dst = _zero_planes(g), _zero_planes(g)
+    ctus = np.ascontiguousarray(ctus)
     if kind == "sao":
-        nc = 3 if g.chromaFormat else 1
-        for i in range(n):
-            for c in range(nc):
-                t = int(ctus["type"][i, c])
-                if t != 255 and t > 4: out.append(f"CTU {i} type {t}")
-                if t == 4 and ctus["band"][i, c] > 31: out.append(f"CTU {i} band {ctus['band'][i, c]}")
-        if vb is not None:
-            if not (0 <= vb.numVer <= 3 and 0 <= vb.numHor <= 3): out.append("virtual boundary count")
-            else:
-                out += [f"vertical VB {vb.posX[k]}" for k in range(vb.numVer) if not (0 < vb.posX[k] < g.width and vb.posX[k] % 8 == 0)]
-                out += [f"horizontal VB {vb.posY[k]}" for k in range(vb.numHor) if not (0 < vb.posY[k] < g.height and vb.posY[k] % 8 == 0)]
-        return out
-    T = tables
-    nL, nC, nCc = T["lumaCoeff"].shape[0], T["chromaCoeff"].shape[0], [T["cc"][c].shape[0] for c in range(2)]
-    if not 16 <= nL <= 24: out.append(f"numLumaSets {nL}")
-    if nC < 0: out.append(f"numChromaAlts {nC}")
-    out += [f"numCc[{c}] {nCc[c]}" for c in range(2) if nCc[c] < 0]
-    for i in range(n):
-        a = ctus[i]
-        f, cx, cy = int(a["enable"][0]), i % ctusW, i // ctusW
-        if f & 0x80 or int(a["enable"][1]) & ~3 or int(a["enable"][2]) & ~3: out.append(f"CTU {i} enable bits")
-        if f & 1 and a["lumaSet"] >= nL: out.append(f"CTU {i} lumaSet {a['lumaSet']}")
-        for c in range(2):
-            if a["enable"][1 + c] & 1 and a["chromaAlt"][c] >= nC: out.append(f"CTU {i} chromaAlt[{c}] {a['chromaAlt'][c]}")
-            if a["ccIdx"][c] > nCc[c]: out.append(f"CTU {i} ccIdx[{c}] {a['ccIdx'][c]}")
-            if a["enable"][1 + c] & 2 and a["ccIdx"][c]: out.append(f"CTU {i} PAD_WIDE with CC-ALF")
-        if f & 32 and (f & (ALF_CLIP_TOP_ | ALF_CLIP_LEFT_) or cx == 0 or cy == 0): out.append(f"CTU {i} PAD_TL")
-        if f & 64 and (f & (ALF_CLIP_BOTTOM_ | ALF_CLIP_RIGHT_) or cx == ctusW - 1 or cy == ctusH - 1): out.append(f"CTU {i} PAD_BR")
-    return out
+        msg = library_refusal("b200_sao_picture", C.byref(g), abi.plane_ptrs(src), abi.plane_ptrs(dst), ctus.ctypes.data, None if vb is None else C.addressof(vb))
+    else:
+        n = [tables["lumaCoeff"].shape[0], tables["chromaCoeff"].shape[0], tables["cc"][0].shape[0], tables["cc"][1].shape[0]]
+        t = dict(lumaCoeff=np.zeros((n[0], 1300), np.int16), chromaCoeff=np.zeros((n[1], 7), np.int16), cc=[np.zeros((m, 7), np.int16) for m in n[2:]])
+        t["lumaClip"], t["chromaClip"] = t["lumaCoeff"], t["chromaCoeff"]
+        T = abi.make_alf_tables(t)
+        msg = library_refusal("b200_alf_picture", C.byref(g), abi.plane_ptrs(src), abi.plane_ptrs(dst), ctus.ctypes.data, C.byref(T))
+    return [] if msg is None else [msg]
