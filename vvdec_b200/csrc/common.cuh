@@ -151,13 +151,7 @@ struct McLaunch {
   int32_t* dmvrMv;                  // device or null
   const b200_wp* wp = nullptr;      // device: explicit weighted prediction entries, or null
   const b200_lmcs* lmcs = nullptr;  // device copy of the LMCS tables: luma predictions are stored forward-mapped; null = LMCS off
-  // TMA descriptors of the picture buffers (device array, 128 B each, 3 per buffer: Y box 24x23, Cb / Cr box 16x11 — the footprints of a 16x16 tile), and
-  // the buffer behind each DPB slot; null: the tiles copy their windows with LDGSTS
-  const void* tmaps = nullptr; uint8_t tmapBuf[B200_MAX_SLOTS] = {};
 };
-// encodes the descriptors for `nBufs` picture buffers (host call, driver entry point cuTensorMapEncodeTiled); returns 0 and leaves *out null if the geometry does not
-// qualify (row pitches that are not multiples of 16 bytes)
-int make_mc_tensor_maps(const b200_geom& g, int16_t* const* bufPlanes /* [nBufs * 3] */, int nBufs, void** out);
 int launch_mc(const McLaunch& L, StreamSet& ss, KProf* prof = nullptr);
 int mc_launch_count(const McLaunch& L);
 int k1_launch_count(const K1Launch& L);

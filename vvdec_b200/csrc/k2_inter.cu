@@ -17,7 +17,6 @@
 #include "vvc_tables.h"
 #include "common.cuh"
 #include <algorithm>
-#include <cuda.h>            // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint, libcuda is not linked)
 
 namespace b200 {
 
@@ -33,33 +32,7 @@ struct McParams {
   int32_t* dmvrMv;
   const b200_wp* wp;                         // explicit weighted prediction entries (b200_pu::wpIdx), or null
   const b200_lmcs* lmcs; int lmcsLog2;       // LMCS: luma predictions are stored forward-mapped (DecCu.cpp:458-476); null = off
-  const CUtensorMap* tmaps; uint8_t tmapBuf[B200_MAX_SLOTS];   // TMA descriptors [buffer * 3 + component] and the buffer of each slot (McLaunch)
 };
-
-// ---- TMA (cp.async.bulk.tensor): the (tw+8) x (th+7) luma and the chroma footprints of an interior 16x16 tile arrive as one bulk tensor copy each, issued
-// by one thread and counted on an mbarrier; the other 63 threads go straight to the wait.  Boxes: Y 24x23, Cb / Cr 16x11 samples (rows of 48 / 32 bytes).
-constexpr int TMA_LW = 24, TMA_LH = 23, TMA_CW = 16, TMA_CH = 11;
-constexpr int TMA_LWIN = 576, TMA_CWIN = 192;                  // window sizes in samples, padded to 128 bytes (the destination alignment of a tensor copy)
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, int count)
-{
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory");
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, int bytes)
-{
-  asm volatile("mbarrier.arrive.expect_tx.release.cta.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, int parity)
-{
-  asm volatile("{\n\t.reg .pred P1;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t@P1 bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
-               :: "r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* smemDst, const CUtensorMap* map, int x, int y, unsigned long long* bar)
-{
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               :: "r"(smem_u32(smemDst)), "l"(map), "r"(x), "r"(y), "r"(smem_u32(bar)) : "memory");
-}
 
 // asynchronous 4-byte global -> shared copies (LDGSTS): a tile issues its whole footprint without waiting on any load, then waits once
 __device__ __forceinline__ void cp_async4(void* smemDst, const void* gmemSrc)
@@ -161,14 +134,8 @@ constexpr int HS = 16, CHS = 8;   // constant row strides of the H-filtered arra
 constexpr int DMVR_TAIL = 1640;   // DMVR scratch behind the windows: bilinear 20x20 x2 + their 1-sample-shifted copies (1600), later the
                                   // shifted final windows (2 x 552 luma, 4 x 132 chroma)
 
-__host__ __device__ inline int mc_smem_elems(int mode, int n, bool tma = false)   // n = tw*th; worst case over the shapes of that size
+__host__ __device__ inline int mc_smem_elems(int mode, int n)   // n = tw*th; worst case over the shapes of that size
 {
-  if (tma) {                                                                // 16x16 tiles with TMA windows (modes 0..2): padded windows first
-    const int lists = mode == 0 ? 1 : 2;
-    int e = lists * (TMA_LWIN + 23 * HS + 2 * (TMA_CWIN + 11 * CHS));
-    if (mode >= 2) e = max(e, 8 * n) + 2 * 324;
-    return (e + 64 + 64) & ~7;                                              // + alignment slack
-  }
   // window (tw+8)x(th+7): 16x16 -> 24x23; 128 -> 24x15 | 16x23; 64 -> 12x23; 32 -> 12x15.  hf: (th+7)*HS.
   const int win = n == 256 ? 552 : n == 128 ? 368 : n == 64 ? 276 : 180;
   const int hf  = (n == 256 ? 23 : n == 128 ? 23 : n == 64 ? 23 : 15) * HS;
@@ -184,8 +151,8 @@ __host__ __device__ inline int mc_smem_elems(int mode, int n, bool tma = false) 
 }
 
 // OPT: luma outputs per thread (1: blockDim = tw*th; 4: blockDim = tw*th/4, each thread filters 4 adjacent samples so that 11 loads feed 32 MACs)
-template <int MODE, int OPT, bool TMA>
-__device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, int16_t* smem, unsigned* sSad, int* sDec, int (*sVxy)[2], unsigned long long* sBar)
+template <int MODE, int OPT>
+__device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, int16_t* smem, unsigned* sSad, int* sDec, int (*sVxy)[2])
 {
   const int tid = threadIdx.x, nthr = blockDim.x;
   const b200_pu& pu = P.pus[tile >> 6];
@@ -205,7 +172,7 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
   const b200_wp* we = (MODE <= 1 && P.wp && pu.wpIdx) ? P.wp + pu.wpIdx - 1 : nullptr;   // explicit weights (never with BDOF / DMVR)
   const bool geo = MODE == 1 && (flags & B200_PU_GEO);      // geometric partitioning: the two 'lists' are the two partitions' uni-predictions
   const int gl2w = 31 - __clz(puW), gl2h = 31 - __clz(puH);
-  const int WS = tw + 8, CS = TMA ? TMA_CW : cw + 4;         // window strides: even, so a row is a run of 32-bit words (TMA: the box widths)
+  const int WS = tw + 8, CS = cw + 4;                        // window strides: even, so a row is a run of 32-bit words
 
   // ---- shared memory carve-up (strides depend on the tile shape) ----
   TileSmem S;
@@ -213,39 +180,22 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
   {
     int16_t* q = smem;
     const int win = WS * (th + 7), hf = (th + 7) * HS, cwin = CS * (ch + 3), chf = (ch + 3) * CHS;
-    if (TMA) {                                               // windows first, each on a 128-byte boundary (tensor copy destinations)
-      q += ((128 - (smem_u32(smem) & 127)) & 127) >> 1;      // the dynamic segment starts behind the kernel's static shared variables
-#pragma unroll
-      for (int l = 0; l < NL; l++) { S.w[l] = q; q += TMA_LWIN; }
-#pragma unroll
-      for (int l = 0; l < NL; l++)
-#pragma unroll
-        for (int c = 0; c < 2; c++) { S.cw[l][c] = q; q += TMA_CWIN; }
-#pragma unroll
-      for (int l = 0; l < NL; l++) { S.h[l] = q; q += hf; }
-#pragma unroll
-      for (int l = 0; l < NL; l++)
-#pragma unroll
-        for (int c = 0; c < 2; c++) { S.chf[l][c] = q; q += chf; }
-    } else {
 #pragma unroll
     for (int l = 0; l < NL; l++) { S.w[l] = q; q += win; S.h[l] = q; q += hf; }
 #pragma unroll
     for (int l = 0; l < NL; l++)
 #pragma unroll
       for (int c = 0; c < 2; c++) { S.cw[l][c] = q; q += cwin; S.chf[l][c] = q; q += chf; }
-    }
     if (MODE == 3 && q < smem + 2 * 441) q = smem + 2 * 441;
     if (MODE >= 2) { if (q < smem + 8 * tw * th) q = smem + 8 * tw * th; if (MODE == 3) { tail = q; q += DMVR_TAIL; } S.p[0] = q; S.p[1] = q + 324; }
   }
 
   // ---- per-list reference planes and motion ----
-  const int16_t* rp[NL][3]; int mvx[NL], mvy[NL]; int tbuf[NL];
+  const int16_t* rp[NL][3]; int mvx[NL], mvy[NL];
 #pragma unroll
   for (int li = 0; li < NL; li++) {
     const int l = BI ? li : l0;
     const int slot = pu.refSlot[l];
-    if (TMA) tbuf[li] = P.tmapBuf[slot];
 #pragma unroll
     for (int c = 0; c < 3; c++) rp[li][c] = P.refs[slot * 3 + c];
     mvx[li] = pu.mv[l][0]; mvy[li] = pu.mv[l][1];
@@ -463,7 +413,6 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
   // Interior tiles (the footprint lies inside the picture and no DMVR window clamp applies) copy whole 32-bit words, 16 lanes per luma
   // row / 8 lanes per chroma row; the footprint's first sample then sits at index wofs (0/1) of each shared row.  Boundary tiles take
   // the per-sample path with clamped coordinates (= the reference's border extension / padded DMVR window).
-  bool tmaAny = false;
   if (!(MODE == 3 && dmvrFast)) {
     const int warp = tid >> 5, lane = tid & 31, nw = max(1, nthr >> 5);
     bool lfast[NL], cfastv[NL];
@@ -472,27 +421,12 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
       lfast[li] = P.fastOk && ox[li] >= 4 && ox[li] + tw + 4 < W && oy[li] >= 3 && oy[li] + th + 3 < H;
       cfastv[li] = chroma && P.fastOk && ocx[li] >= 2 && ocx[li] + cw + 2 < CWp && ocy[li] >= 1 && ocy[li] + ch + 1 < CHp;
       if (MODE == 3) { lfast[li] = lfast[li] && wx1[li][0] == (1 << 20); cfastv[li] = cfastv[li] && wx1[li][1] == (1 << 20); }
-      tmaAny = tmaAny || lfast[li] || cfastv[li];
-    }
-    if (TMA && tmaAny && tid == 0) {
-      // interior footprints: one tensor copy per window (the boxes may hang over the right / bottom picture edge in their padding columns only: zero fill)
-      int bytes = 0;
-#pragma unroll
-      for (int li = 0; li < NL; li++) bytes += (lfast[li] ? TMA_LW * TMA_LH * 2 : 0) + (cfastv[li] ? 2 * TMA_CW * TMA_CH * 2 : 0);
-      mbar_expect_tx(sBar, bytes);
-#pragma unroll
-      for (int li = 0; li < NL; li++) {
-        const CUtensorMap* tm = P.tmaps + tbuf[li] * 3;
-        if (lfast[li]) tma_load_2d(S.w[li], tm, ox[li] - 3, oy[li] - 3, sBar);
-        if (cfastv[li]) { tma_load_2d(S.cw[li][0], tm + 1, ocx[li] - 1, ocy[li] - 1, sBar); tma_load_2d(S.cw[li][1], tm + 2, ocx[li] - 1, ocy[li] - 1, sBar); }
-      }
     }
 #pragma unroll
     for (int li = 0; li < NL; li++) {
       const bool fast = lfast[li];
-      wofs[li] = (fast && !TMA) ? ((ox[li] - 3) & 1) : 0;
-      if (fast && TMA) {
-      } else if (fast) {
+      wofs[li] = fast ? ((ox[li] - 3) & 1) : 0;
+      if (fast) {
         const int half = lane >> 4, wl = lane & 15, rw = rs0 >> 1;
         const uint32_t* src = reinterpret_cast<const uint32_t*>(rp[li][0] + (size_t)(oy[li] - 3) * rs0 + ((ox[li] - 3) & ~1)) + (size_t)(warp * 2 + half) * rw + wl;
         uint32_t* dst = reinterpret_cast<uint32_t*>(S.w[li]) + (warp * 2 + half) * (WS >> 1) + wl;
@@ -510,9 +444,8 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
       cofs[li] = 0;
       if (chroma) {
         const bool cfast = cfastv[li];
-        cofs[li] = (cfast && !TMA) ? ((ocx[li] - 1) & 1) : 0;
-        if (cfast && TMA) {
-        } else if (cfast) {
+        cofs[li] = cfast ? ((ocx[li] - 1) & 1) : 0;
+        if (cfast) {
           const int sub = lane >> 3, wl = lane & 7, rwc = rs1 >> 1, npc = (ch + 6) >> 2;   // 4 rows per pass, npc passes per component
           const size_t cbase = (size_t)(ocy[li] - 1) * rs1 + ((ocx[li] - 1) & ~1);
           for (int q = warp; q < 2 * npc; q += nw) {
@@ -536,7 +469,6 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
     }
   }
   cp_async_wait_all();
-  if (TMA && tmaAny) mbar_wait(sBar, 0);
   __syncthreads();
 
   // ================================================================ stage B: horizontal filters
@@ -729,17 +661,15 @@ __device__ __forceinline__ void mc_tile(const McParams& P, const uint32_t tile, 
 
 // One CTA per entry of one tile list (bucket.cu); the host sizes the grid from the list length it reads back after bucketing, and the
 // hardware scheduler balances the lists of all streams.
-template <int MODE, int OPT, bool TMA>
+template <int MODE, int OPT>
 __global__ void __launch_bounds__(64, MODE >= 2 ? 12 : 16) mc_kernel(const McParams P, const int list)
 {
   extern __shared__ __align__(128) int16_t smem[];
   __shared__ unsigned sSad[25];
   __shared__ int sDec[3];
   __shared__ int sVxy[16][2];
-  __shared__ __align__(8) unsigned long long sBar;
   if ((int)blockIdx.x >= P.meta[LM_CNT + list]) return;
-  if (TMA) { if (threadIdx.x == 0) mbar_init(&sBar, 1); __syncthreads(); }
-  mc_tile<MODE, OPT, TMA>(P, P.tiles[P.meta[LM_OFF + list] + blockIdx.x], smem, sSad, sDec, sVxy, &sBar);
+  mc_tile<MODE, OPT>(P, P.tiles[P.meta[LM_OFF + list] + blockIdx.x], smem, sSad, sDec, sVxy);
 }
 
 // ------------------------------------------------------------------------------------------------ affine tiles (xPredAffineBlk :934)
@@ -944,37 +874,25 @@ int launch_mc(const McLaunch& L, StreamSet& ss, KProf* prof)
   P.pus = L.pus; P.dmvrMv = L.dmvrMv; P.tiles = L.tiles; P.meta = L.meta;
   P.wp = L.wp;
   P.lmcs = L.lmcs; P.lmcsLog2 = 0; { int o = (1 << L.geom.bitDepth) / 16; while ((1 << (P.lmcsLog2 + 1)) <= o) P.lmcsLog2++; }
-  P.tmaps = reinterpret_cast<const CUtensorMap*>(L.tmaps); memcpy(P.tmapBuf, L.tmapBuf, sizeof(P.tmapBuf));
-  // The tensor-copy windows are OFF unless B200_MC_TMA=1: LDGSTS windows are the default path, the one the test suite runs and the benchmark times.
-  // The TMA path (tools/tma_probe.cu exercises the same descriptors stand-alone) has not been validated on sm_90a.
-  static const bool tmaEnv = getenv("B200_MC_TMA") && !strcmp(getenv("B200_MC_TMA"), "1");
-  const bool tmaOn = P.tmaps && P.chroma && tmaEnv;
   int launched = 0;
   if (prof) prof->begin(B200_KF_MC_TILE, ss.main);
   for (int m = 3; m >= 0; m--) for (int k = 3; k >= 0; k--) {      // heaviest lists first (DMVR 16x16 ... uni 8x4)
     const int nsamp = 32 << k, list = m * 4 + k, grid = L.cnt[list];
     if (!grid || (m >= 2 && k < 2)) continue;                       // BDOF / DMVR tiles have at least 128 samples (bucket.cu rejects others)
     cudaStream_t s = ss.pick(launched++);
-    const bool tma = tmaOn && k == 3 && m <= 2;               // 16x16 tiles of the uni / bi / BDOF lists: windows by tensor copies
-    const size_t smem = (size_t)mc_smem_elems(m, nsamp, tma) * 2;
-    if (tma) {
-      switch (m) {
-        case 0: mc_kernel<0, 4, true><<<grid, 64, smem, s>>>(P, list); break;
-        case 1: mc_kernel<1, 4, true><<<grid, 64, smem, s>>>(P, list); break;
-        default: mc_kernel<2, 4, true><<<grid, 64, smem, s>>>(P, list); break;
-      }
-    } else if (k >= 2) {     // 128 / 256 samples: 4 luma outputs per thread -> 32 / 64 threads
+    const size_t smem = (size_t)mc_smem_elems(m, nsamp) * 2;
+    if (k >= 2) {            // 128 / 256 samples: 4 luma outputs per thread -> 32 / 64 threads
       const int nthr = nsamp >> 2;
       switch (m) {
-        case 0: mc_kernel<0, 4, false><<<grid, nthr, smem, s>>>(P, list); break;
-        case 1: mc_kernel<1, 4, false><<<grid, nthr, smem, s>>>(P, list); break;
-        case 2: mc_kernel<2, 4, false><<<grid, nthr, smem, s>>>(P, list); break;
-        default: mc_kernel<3, 4, false><<<grid, nthr, smem, s>>>(P, list); break;
+        case 0: mc_kernel<0, 4><<<grid, nthr, smem, s>>>(P, list); break;
+        case 1: mc_kernel<1, 4><<<grid, nthr, smem, s>>>(P, list); break;
+        case 2: mc_kernel<2, 4><<<grid, nthr, smem, s>>>(P, list); break;
+        default: mc_kernel<3, 4><<<grid, nthr, smem, s>>>(P, list); break;
       }
     } else {
       switch (m) {
-        case 0: mc_kernel<0, 1, false><<<grid, nsamp, smem, s>>>(P, list); break;
-        default: mc_kernel<1, 1, false><<<grid, nsamp, smem, s>>>(P, list); break;
+        case 0: mc_kernel<0, 1><<<grid, nsamp, smem, s>>>(P, list); break;
+        default: mc_kernel<1, 1><<<grid, nsamp, smem, s>>>(P, list); break;
       }
     }
     B200_CUDA(cudaGetLastError());
@@ -982,31 +900,6 @@ int launch_mc(const McLaunch& L, StreamSet& ss, KProf* prof)
   if (L.cnt[16]) { cudaStream_t s = ss.pick(launched++); mc_affine_kernel<<<L.cnt[16], 256, 0, s>>>(P); B200_CUDA(cudaGetLastError()); }
   ss.join();
   if (prof) prof->end(B200_KF_MC_TILE, ss.main);      // with forked streams the affine tiles are inside the same interval
-  return 0;
-}
-
-// Tensor maps of the picture buffers: 2-D, 16-bit elements, no swizzle / interleave, zero fill outside (never read: TMA windows are interior footprints).
-int make_mc_tensor_maps(const b200_geom& g, int16_t* const* bufPlanes, int nBufs, void** out)
-{
-  *out = nullptr;
-  if (g.chromaFormat != 1 || (g.stride[0] & 7) || (g.stride[1] & 7) || (g.stride[2] & 7)) return 0;      // global strides must be multiples of 16 bytes
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                               CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  void* fn = nullptr; cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn) { cudaGetLastError(); return 0; }
-  std::vector<CUtensorMap> maps((size_t)nBufs * 3);
-  for (int i = 0; i < nBufs * 3; i++) {
-    const int c = i % 3;
-    if ((uintptr_t)bufPlanes[i] & 15) return 0;
-    const cuuint64_t dims[2] = {(cuuint64_t)(c ? g.width >> 1 : g.width), (cuuint64_t)(c ? g.height >> 1 : g.height)};
-    const cuuint64_t strides[1] = {(cuuint64_t)g.stride[c] * 2};
-    const cuuint32_t box[2] = {(cuuint32_t)(c ? TMA_CW : TMA_LW), (cuuint32_t)(c ? TMA_CH : TMA_LH)}, estr[2] = {1, 1};
-    const CUresult r = reinterpret_cast<EncodeFn>(fn)(&maps[i], CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, bufPlanes[i], dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return 0;
-  }
-  B200_CUDA(cudaMalloc(out, maps.size() * sizeof(CUtensorMap)));
-  B200_CUDA(cudaMemcpy(*out, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
   return 0;
 }
 

@@ -455,8 +455,9 @@ __global__ void __launch_bounds__(IT_THREADS, 12) intra_kernel(const IntraParams
 // flags for earlier blocks of its own CTU and on the global done words only for blocks of the neighbouring CTUs (left, above-left, above, above-right:
 // all earlier in the wave front, so the oldest unfinished block never waits on a block that has not been started — no deadlock at any residency).
 // Samples are written through: to the shared tile for the CTU's own later blocks, to the plane for the other CTUs and the in-loop filters.
-// a block is worked on by a group of V2_GROUP threads, V2_GROUPS blocks of the CTU at a time (template parameters of the kernel: the chains of an intra CTU
-// are Y -> Y -> Y, Cb -> Cb, Cr -> Cr, so about three blocks can run at once and the latency of one block is what counts)
+// a block is worked on by a group of V2_GROUP threads, V2_GROUPS blocks of the CTU at a time (the chains of an intra CTU are Y -> Y -> Y, Cb -> Cb,
+// Cr -> Cr, so about three blocks can run at once and the latency of one block is what counts)
+constexpr int V2_GROUP = 128, V2_GROUPS = 5, V2_THREADS = V2_GROUP * V2_GROUPS;
 constexpr int V2_LS = 136, V2_CS = 72;                       // tile row pitch in samples: a multiple of 16 bytes (16-byte asynchronous copies), rows 4 banks apart
 constexpr int V2_TILE = 128 * V2_LS + 2 * 64 * V2_CS;        // samples of one tile set (Y, Cb, Cr)
 constexpr int V2_RECS = 1024;                                // records staged in shared memory (a CTU with more blocks reads the rest from global memory)
@@ -464,7 +465,7 @@ constexpr int V2_FLAGS = 128 * 128 / 16 + 2 * (64 * 64 / 4); // most blocks a CT
 static_assert(V2_FLAGS == INTRA_MAX_CTU_BLOCKS, "the documented per-CTU block limit is the number of done bytes");
 struct V2Scratch { int16_t T[2][IT_REF], L[2][IT_REF], M[IT_ARR], S[IT_ARR], Lm[32 * 32], LmTop[64], LmLeft[64]; int LmPar[4]; int next[2], sum; };
 constexpr int V2_OWN = 3 * 32 * 32;                         // owner words of the CTU's units: luma 32 x 32 (4x4 units), Cb / Cr 32 x 32 each (2x2 units)
-constexpr size_t v2_smem(int groups) { return (size_t)2 * V2_TILE * sizeof(int16_t) + groups * sizeof(V2Scratch) + V2_RECS * sizeof(b200_intra_tu) + V2_OWN * sizeof(int) + V2_FLAGS + 64; }
+constexpr size_t V2_SMEM = (size_t)2 * V2_TILE * sizeof(int16_t) + V2_GROUPS * sizeof(V2Scratch) + V2_RECS * sizeof(b200_intra_tu) + V2_OWN * sizeof(int) + V2_FLAGS + 64;
 __device__ __forceinline__ void v2_cp4(void* smemDst, const void* gmemSrc)      // asynchronous 4-byte global -> shared copy (LDGSTS): the whole CTU in flight before one wait
 {
   const unsigned d = (unsigned)__cvta_generic_to_shared(smemDst);
@@ -532,10 +533,8 @@ __device__ unsigned long long gK6Prof[48];
 #define K6P(i, t0) do {} while (0)
 #define K6C(i) do {} while (0)
 #endif
-template <int V2_GROUP, int V2_GROUPS>
-__global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(const IntraParams P, const int* __restrict__ ctuOrder, int* counters)
+__global__ void __launch_bounds__(V2_THREADS, 1) intra_ctu_kernel(const IntraParams P, const int* __restrict__ ctuOrder, int* counters)
 {
-  constexpr int V2_THREADS = V2_GROUP * V2_GROUPS;
   extern __shared__ __align__(16) unsigned char smem[];
   int16_t* tileRec = reinterpret_cast<int16_t*>(smem);
   int16_t* tileRes = tileRec + V2_TILE;
@@ -591,7 +590,7 @@ __global__ void __launch_bounds__(V2_GROUP * V2_GROUPS, 1) intra_ctu_kernel(cons
 
     // ---- the CTU's blocks, one group each, in decoding order
     V2Scratch& SC = scratch[grp];
-#define V2_SYNC() do { if (V2_GROUP == 32) __syncwarp(); else asm volatile("bar.sync %0, %1;" :: "r"(grp + 1), "r"(V2_GROUP) : "memory"); } while (0)
+#define V2_SYNC() asm volatile("bar.sync %0, %1;" :: "r"(grp + 1), "r"(V2_GROUP) : "memory")
     // Block tickets: group g starts with block g (sNext starts past them); while a group works on a block, its lane 0 takes the group's next ticket.  Tickets
     // still go out in decoding order and only to running groups.  The ticket alternates between two words: between lane 0's write of a word and the group's
     // read of it lies the block's last barrier, and between that read and lane 0's next write of the same word the next block's first barrier.
@@ -1022,13 +1021,11 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
       diag = std::max(diag, n);
     }
     const int ctas = (int)std::min<size_t>({nCtu, (size_t)num_sms(), (size_t)(kWaveCtasPerDiag2 * diag + 1) / 2});
-    static const int shape = getenv("B200_INTRA_GROUP") ? atoi(getenv("B200_INTRA_GROUP")) : 0;      // measurement switch: threads per block group
-#define V2_GO(G, N) do { static bool attr = false; if (!attr) { B200_CUDA(cudaFuncSetAttribute(intra_ctu_kernel<G, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)v2_smem(N))); attr = true; } \
-                         intra_ctu_kernel<G, N><<<ctas, G * N, v2_smem(N), s>>>(P, ctuOrder, counters); } while (0)
     // 128x5: 96 registers, no spills (128x6 is capped at 80 and spills).  Single-lane 4K I picture, grid 2x the diagonal, H100 80 GB HBM3 at 400 W:
     // 128x5 9.56 ms, 128x6 9.99 ms
-    if (shape == 1284) V2_GO(128, 4); else if (shape == 32) V2_GO(32, 8); else V2_GO(128, 5);
-#undef V2_GO
+    static bool attr = false;
+    if (!attr) { B200_CUDA(cudaFuncSetAttribute(intra_ctu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)V2_SMEM)); attr = true; }
+    intra_ctu_kernel<<<ctas, V2_THREADS, V2_SMEM, s>>>(P, ctuOrder, counters);
     B200_CUDA(cudaGetLastError());
     return 0;
   }

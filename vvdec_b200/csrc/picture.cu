@@ -60,7 +60,6 @@ struct b200_ctx {
   DevBuf grainStage[2], grainTab;    // b200_get_frame_grain_async: grained copy of the frame, device copies of the tables + block seeds
   DevBuf resiBuf;                    // residual planes of intra CUs (K1 -> K6), allocated with the first picture that carries intra blocks
   DevBuf hashBuf;                    // b200_frame_hash_async: accumulators + digest per ticket
-  void* tmaps = nullptr;             // TMA descriptors of the picture buffers (k2_inter.cu), or null
 
   DevPlanes planes(int buf) const {
     DevPlanes d; char* b = reinterpret_cast<char*>(bufs[buf]);
@@ -102,11 +101,6 @@ B200_API int b200_ctx_create(b200_ctx** out, const b200_geom* g, int numSlots, i
   for (auto& e : c->readDone) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   for (int i = 0; i < numSlots + 2; i++) { B200_CUDA(cudaMalloc(&c->bufs[i], c->picBytes)); B200_CUDA(cudaMemset(c->bufs[i], 0, c->picBytes)); }
   for (int s = 0; s < numSlots; s++) c->slotBuf[s] = s;
-  {
-    std::vector<int16_t*> pl;
-    for (int i = 0; i < numSlots + 2; i++) { DevPlanes d = c->planes(i); for (int k = 0; k < 3; k++) pl.push_back(d.p[k]); }
-    if (int rc = make_mc_tensor_maps(*g, pl.data(), numSlots + 2, &c->tmaps)) return rc;
-  }
   c->work[0] = numSlots; c->work[1] = numSlots + 1;
   c->arenas.resize(numArenas);
   for (auto& A : c->arenas) { B200_CUDA(cudaEventCreateWithFlags(&A.uploaded, cudaEventDisableTiming)); B200_CUDA(cudaEventCreateWithFlags(&A.done, cudaEventDisableTiming)); B200_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&A.hMeta), (2 * LM_INTS + 4) * sizeof(int), cudaHostAllocDefault)); }
@@ -121,7 +115,6 @@ B200_API void b200_ctx_destroy(b200_ctx* c)
   for (auto& A : c->arenas) { cudaEventDestroy(A.uploaded); cudaEventDestroy(A.done); if (A.hMeta) cudaFreeHost(A.hMeta); }
   cudaStreamDestroy(c->upStream);
   for (auto p : c->bufs) cudaFree(p);
-  if (c->tmaps) cudaFree(c->tmaps);
   for (auto e : c->readDone) cudaEventDestroy(e);
   for (auto e : c->ticketEv) cudaEventDestroy(e);
   cudaEventDestroy(c->finalEv); cudaStreamDestroy(c->copyStream);
@@ -301,7 +294,6 @@ B200_API int b200_pic_run(b200_ctx* c, int ai)
     McLaunch L; L.geom = g; L.dst = P; memset(L.refs, 0, sizeof(L.refs));
     for (int sl = 0; sl < c->numSlots; sl++) { DevPlanes d = c->planes(c->slotBuf[sl]); for (int k = 0; k < 3; k++) L.refs[sl * 3 + k] = d.p[k]; }
     for (int k = 0; k < 3; k++) L.refStride[k] = g.stride[k];
-    L.tmaps = c->tmaps; for (int sl = 0; sl < c->numSlots; sl++) L.tmapBuf[sl] = (uint8_t)c->slotBuf[sl];
     L.pus = A.pus; L.tiles = A.tiles; L.meta = A.mcMeta; L.dmvrMv = A.dmvrMv; L.lmcs = A.lmcs; L.wp = A.wp;
     for (int l = 0; l < MC_LISTS; l++) L.cnt[l] = A.hMeta[LM_CNT + l];
     if (int rc = launch_mc(L, c->ss, c->profiling ? &c->prof : nullptr)) return rc;
