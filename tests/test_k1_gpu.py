@@ -126,3 +126,33 @@ def test_k1_explicit_scaling_lists(b200, oracle, seed, W, H, bd):
     c2 = [p.copy() for p in planes]
     oracle.orc_k1_residual(C.byref(g), abi.plane_ptrs(c2), tus2.ctypes.data, len(tus2), coefs, None, 0)
     assert not np.array_equal(a[0], c2[0])
+
+
+def _first_diff(case, want, got):
+    """(plane, y, x, oracle sample, kernel sample, index and tags of the TUs writing it) of the first differing sample, or None."""
+    for c, (a, b) in enumerate(zip(want, got)):
+        if a is None or np.array_equal(a, b): continue
+        y, x = (int(v) for v in np.argwhere(a != b)[0])
+        t = case["tus"]
+        cx, cy = t["x"].astype(int), t["y"].astype(int)
+        on = ((t["comp"] == c) | ((t["ict"] != 0) & (t["comp"] == 3 - c) & (c > 0))) & (cx <= x) & (x < cx + (1 << t["log2w"].astype(int))) & (cy <= y) & (y < cy + (1 << t["log2h"].astype(int)))
+        return c, y, x, int(a[y, x]), int(b[y, x]), [(int(i), case["tags"][i]) for i in np.flatnonzero(on)]
+    return None
+
+
+@pytest.mark.parametrize("mode", [0, 1])
+@pytest.mark.parametrize("name", list(synth.K1_SWEEP_CASES))
+def test_k1_designed_sweep(b200, oracle, name, mode):
+    """Every case of the designed K1 sweep (synth.k1_sweep) through b200_k1_residual, bit-exact against the oracle on every plane; the stride padding keeps
+    its sentinel.  A failure names the first differing sample and the TU(s) that write it."""
+    case = synth.k1_sweep(name)
+    g, tus, coefs, sl = case["g"], case["tus"], case["coefs"], case["scaling"]
+    want, got = case["planes"], [None if p is None else p.copy() for p in case["planes"]]
+    oracle.orc_k1_residual(C.byref(g), abi.plane_ptrs(want), tus.ctypes.data, len(tus), coefs, None if sl is None else sl.ctypes.data, mode)
+    vvdec_b200.check(b200.b200_k1_residual(C.byref(g), abi.plane_ptrs(got), tus.ctypes.data, len(tus), coefs.ctypes.data, len(coefs),
+                                            None if sl is None else sl.ctypes.data, 0 if sl is None else len(sl), mode))
+    diff = _first_diff(case, want, got)
+    assert diff is None, f"{name} mode {mode}: plane {diff[0]} (y {diff[1]}, x {diff[2]}): oracle {diff[3]}, kernel {diff[4]}; TU {diff[5]}"
+    for c, p in enumerate(got):
+        if p is not None and p.shape[1] > (case["W"] >> (c > 0)):
+            assert (p[:, case["W"] >> (c > 0):] == -7).all(), f"{name}: stride padding of plane {c} written"

@@ -4,7 +4,7 @@ Pattern = vvdec_unit_test.cpp:221-303 (same call on `ref` and `opt`, random + co
 import ctypes as C
 import numpy as np
 import pytest
-from vvdec_b200 import abi
+from vvdec_b200 import abi, synth
 from tests.helpers import RefTuSyntax, aligned, aligned_copy
 
 pytestmark = pytest.mark.ref
@@ -241,3 +241,29 @@ def test_tu_level_isp_thin_partitions(oracle, ref):
         rec = _tu_case(oracle, ref, s, lv)
         seen.add((rec.log2w, rec.log2h, rec.trType))
     assert any(k[0] == 0 for k in seen) and any(k[1] == 0 for k in seen) and len({k[2] for k in seen}) >= 3
+
+
+@pytest.mark.parametrize("name", [n for n, v in synth.K1_SWEEP_CASES.items() if v[0] != "random"])
+def test_k1_sweep_tus_match_the_reference(oracle, ref, name):
+    """Every TU of the designed K1 sweep that has a syntax form goes through the glue's flattener and the reference's invTransformNxN
+    (+ invTransformICT): the flattened record equals the sweep's field for field, and the reference's residual equals the oracle's on both planes.
+    The others (level corners of part of a coefficient group, inputs past LFNST's zero-out size, 2-sample sides in luma, pairs only SBT gives, ...) are
+    records only the record interface allows; the kernel is checked on them against the oracle (tests/test_k1_gpu.py)."""
+    case = synth.k1_sweep(name)
+    pinned = 0
+    for i, (t, syn) in enumerate(zip(case["tus"], case["syntax"])):
+        if syn is None: continue
+        s = RefTuSyntax()
+        for k, v in syn.items(): setattr(s, k, v)
+        w, h = 1 << int(t["log2w"]), 1 << int(t["log2h"])
+        s.maxScanPosX, s.maxScanPosY = int(t["maxX"]), int(t["maxY"])
+        lv = np.zeros((h, w), np.int16)
+        c = synth.k1_corner(case["tus"], case["coefs"], i)
+        lv[:c.shape[0], :c.shape[1]] = c
+        rec = _tu_case(oracle, ref, s, lv.reshape(-1).copy())
+        got = {f: getattr(rec, f) for f in ("log2w", "log2h", "comp", "flags", "maxX", "maxY", "trType", "lfnst", "ict", "rightShift", "inBits", "scale")}
+        want = {f: int(t[f]) for f in got}
+        assert got == want, (name, i, case["tags"][i], {f: (got[f], want[f]) for f in got if got[f] != want[f]})
+        pinned += 1
+    print(f"{name}: {pinned} TUs pinned to the reference, {len(case['tus']) - pinned} record-only")
+    assert pinned > len(case["tus"]) // 3

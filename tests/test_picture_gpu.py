@@ -534,3 +534,43 @@ def test_sao_alf_picture_refusals(b200, oracle, what, bad, fixed):
     assert err is not None and b"b200_pic_upload" in err, (what, err, ok)
     err, ok = _filter_picture(b200, oracle, case, fixed.get("strides"), case["ctus"], alf, flags=flags, bd=fixed.get("bd", 10))
     assert err is None and ok is True, (what, err, ok)
+
+
+@pytest.mark.parametrize("ctu", [32, 64, 128])
+def test_k1_lmcs_chroma_scaling_in_a_picture(b200, oracle, ctu):
+    """K1's LMCS passes on the picture path (luma TUs, then the per-VPDU chroma scale, then chroma TUs scaled by their VPDU's entry; blocks of 4 samples
+    unscaled, joint-CbCr partners scaled): synth.k1_lmcs_picture's TUs over a `given` prediction, no PUs, deblocking / SAO / ALF off.  The VPDUs use at
+    least three different scales besides the neutral one, and the picture matches the oracle chain."""
+    W, H, bd = 256, 128, 10
+    g = abi.make_geom(W, H, bd, ctu=ctu)
+    tus, coefs, given, tags = synth.k1_lmcs_picture(ctu, W, H, bd)
+    pic = synth.gen_picture(np.random.default_rng(ctu), W, H, bd, ctu=ctu, dst_slot=4, inter=False, tu_kw=dict(p_cbf=0.0), deblock=False, sao=False,
+                            alf=False, lmcs=True)
+    st = pic["struct"]
+    assert st.flags == abi.PIC_LMCS and pic["lmcs"]["struct"].chromaAdj
+    pic["tus"], pic["coefs"], pic["given"] = tus, coefs, given
+    st.tus, st.numTus, st.coefs, st.numCoefs = tus.ctypes.data, len(tus), coefs.ctypes.data, len(coefs)
+    for c in range(3): st.given[c] = given[c].ctypes.data
+    # the VPDU scales the chroma TUs see: the luma plane after the luma TUs
+    luma = [given[0].copy(), None, None]
+    ly = np.ascontiguousarray(tus[tus["comp"] == 0])
+    oracle.orc_k1_residual(C.byref(g), abi.plane_ptrs(luma), ly.ctypes.data, len(ly), coefs, None, 0)
+    vs = 64 if ctu == 128 else ctu
+    scale = np.zeros((W // vs) * (H // vs), np.int32)
+    oracle.orc_lmcs_vpdu_scales(C.byref(g), luma[0], C.byref(pic["lmcs"]["struct"]), scale.ctypes.data)
+    assert len(set(scale.tolist()) - {2048}) >= 3, scale
+    dpb = [[np.zeros_like(p) for p in given] for _ in range(4)]
+    want, _ = oracle_decompress(oracle, g, dpb, pic)
+    ctx = C.c_void_p()
+    vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 2, -1))
+    try:
+        h = b200.b200_decompress_picture(ctx, C.byref(st))
+        assert h >= 0, b200.b200_last_error()
+        vvdec_b200.check(b200.b200_wait_picture(ctx, h, None, 0))
+        got = [np.zeros_like(p) for p in want]
+        vvdec_b200.check(b200.b200_get_frame(ctx, 4, abi.plane_ptrs(got)))
+        for c in range(3):
+            bad = np.argwhere(want[c] != got[c])
+            assert len(bad) == 0, f"CTU {ctu}: plane {c}: {len(bad)} diffs, first at {bad[:1].tolist()}"
+    finally:
+        b200.b200_ctx_destroy(ctx)

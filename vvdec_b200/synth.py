@@ -54,6 +54,20 @@ def _laplace_levels(rng, n, heavy=False):
     return np.clip(np.rint(v), -32768, 32767).astype(np.int16)
 
 
+TU_INV_SCALES = ((40, 45, 51, 57, 64, 72), (57, 64, 72, 80, 90, 102))      # g_invQuantScales: [sqrt2 shape][QP % 6]
+
+
+def tu_dequant(qp, bit_depth, l2w, l2h, ts=False, dep_quant=False, scaling=False):
+    """(rightShift, inBits, scale) of a TU record, as the flattener derives them (vvdec_glue/flatten_tu.h): qp = QP' (QP + 6 (bitDepth - 8)),
+    at least 4 under transform skip; dependent quantisation adds 1 to QP and to the shift, explicit scaling lists add 4 to the shift."""
+    sqrt2 = (not ts) and ((l2w + l2h) & 1)
+    q = max(qp, 4) if ts else qp
+    per, rem = ((q + 1) // 6, (q + 1) % 6) if dep_quant else (q // 6, q % 6)
+    tr_shift = 15 - bit_depth - ((l2w + l2h) >> 1) + (-1 if sqrt2 else 0)
+    right_shift = 6 + (1 if dep_quant else 0) - ((0 if ts else tr_shift) + per) + (4 if scaling else 0)
+    return right_shift, min(16, 32 + right_shift - 7), TU_INV_SCALES[1 if sqrt2 else 0][rem]
+
+
 def gen_tus(rng, cus, bit_depth=10, p_cbf=0.5, p_mts=0.2, p_lfnst=0.1, p_ts=0.05, p_bdpcm=0.03, p_jccr=0.1,
             p_full=0.3, chroma=True, heavy=0.02, dep_quant=True, p_intra=0.15, scaling=None):
     """TU records + packed level arena for a CU list (one TU per <=64x64 tile of each CU, all 3 components).
@@ -62,7 +76,6 @@ def gen_tus(rng, cus, bit_depth=10, p_cbf=0.5, p_mts=0.2, p_lfnst=0.1, p_ts=0.05
     B200_TU_SCALING, slOff -> the table of their (log2w, log2h), right shift + 4."""
     recs, coefs = [], []
     ncoef = 0
-    inv_scales = np.array([[40, 45, 51, 57, 64, 72], [57, 64, 72, 80, 90, 102]])
     for (cx, cy, cw, ch) in cus:
         if rng.random() >= p_cbf:
             continue
@@ -115,16 +128,11 @@ def gen_tus(rng, cus, bit_depth=10, p_cbf=0.5, p_mts=0.2, p_lfnst=0.1, p_ts=0.05
                             maxX = min(limx, (maxX // cgw + 1) * cgw) - 1
                             maxY = min(limy, (maxY // cgh + 1) * cgh) - 1
                     is_ts = bool(flags & abi.TU_TS)
-                    sqrt2 = (not is_ts) and ((l2w + l2h) & 1)
-                    dq = dep_quant and not is_ts
-                    q = max(qp, 4) if is_ts else qp
-                    per, rem = ((q + 1) // 6, (q + 1) % 6) if dq else (q // 6, q % 6)
-                    tr_shift = 15 - bit_depth - ((l2w + l2h) >> 1) + (-1 if sqrt2 else 0)
-                    right_shift = 6 + (1 if dq else 0) - ((0 if is_ts else tr_shift) + per)
                     sl_off = 0
-                    if scaling is not None and not is_ts and not lfnst:
-                        flags |= abi.TU_SCALING; right_shift += 4; sl_off = scaling["off"][(l2w, l2h)]
-                    in_bits = min(16, 32 + right_shift - 7)
+                    use_sl = scaling is not None and not is_ts and not lfnst
+                    if use_sl:
+                        flags |= abi.TU_SCALING; sl_off = scaling["off"][(l2w, l2h)]
+                    right_shift, in_bits, scale = tu_dequant(qp, bit_depth, l2w, l2h, is_ts, dep_quant and not is_ts, use_sl)
                     n = (maxX + 1) * (maxY + 1)
                     lv = _laplace_levels(rng, n, rng.random() < heavy)
                     if lfnst:
@@ -132,8 +140,7 @@ def gen_tus(rng, cus, bit_depth=10, p_cbf=0.5, p_mts=0.2, p_lfnst=0.1, p_ts=0.05
                         yy, xx = np.divmod(np.arange(n), maxX + 1)
                         lv[(xx + yy) > 2] = 0
                     if lv[-1] == 0: lv[-1] = 1
-                    recs.append((x, y, l2w, l2h, comp, flags, maxX, maxY, tr, lfnst, ict, right_shift, in_bits,
-                                 int(inv_scales[1 if sqrt2 else 0][rem]), ncoef, sl_off, (0, 0)))
+                    recs.append((x, y, l2w, l2h, comp, flags, maxX, maxY, tr, lfnst, ict, right_shift, in_bits, scale, ncoef, sl_off, (0, 0)))
                     coefs.append(lv); ncoef += n
     tus = np.array(recs, dtype=abi.TU_DTYPE) if recs else np.zeros(0, abi.TU_DTYPE)
     arena = np.concatenate(coefs) if coefs else np.zeros(0, np.int16)
@@ -2161,3 +2168,294 @@ def k45_record_problems(kind, g, ctus, tables=None, vb=None):
         T = abi.make_alf_tables(t)
         msg = library_refusal("b200_alf_picture", C.byref(g), abi.plane_ptrs(src), abi.plane_ptrs(dst), ctus.ctypes.data, C.byref(T))
     return [] if msg is None else [msg]
+
+
+def k1_record_problems(g, tus, coefs, scaling=None):
+    """What b200_k1_residual says about a geometry, its TU records, level arena and scaling arena: [] when it accepts the call, else [its error message]."""
+    planes, tus, coefs = _zero_planes(g), np.ascontiguousarray(tus), np.ascontiguousarray(coefs, np.int16)
+    sl = None if scaling is None else np.ascontiguousarray(scaling, np.int32)
+    msg = library_refusal("b200_k1_residual", C.byref(g), abi.plane_ptrs(planes), tus.ctypes.data, len(tus), coefs.ctypes.data, len(coefs),
+                          None if sl is None else sl.ctypes.data, 0 if sl is None else len(sl), 0)
+    return [] if msg is None else [msg]
+
+
+# ---- K1: the designed residual sweep (tests/test_k1_*.py).  Each TU names what it is there for (tags) and, where the decoder can produce it, the
+# syntax it comes from (tests.helpers.RefTuSyntax fields; tests/test_k1_oracle_vs_ref.py flattens it with the glue and runs it through the reference).
+K1_TR_NAMES = {abi.TR_DCT2: "DCT2", abi.TR_DST7: "DST7", abi.TR_DCT8: "DCT8"}
+K1_ODD = (1, 3, 5, 15, 31)
+K1_SCAN = ((0, 0), (0, 1), (1, 0), (0, 2), (1, 1), (2, 0), (0, 3), (1, 2), (2, 1), (3, 0), (1, 3), (2, 2), (3, 1), (2, 3), (3, 2), (3, 3))   # (y, x) of the 16 LFNST inputs
+# LFNST (set, transpose) -> an intra mode that selects it on a square block (H.266 lfnstTrSetIdx; modes above 34 transpose)
+K1_LFNST_MODES = {(0, 0): 0, (1, 0): 8, (1, 1): 60, (2, 0): 18, (2, 1): 50, (3, 0): 34, (3, 1): 40}
+# (zeroOutSize, outputs) -> the shapes with that LFNST form; the second list holds the dual-tree chroma shapes
+K1_LFNST_SHAPES = {(8, 16): ([(4, 4)], [(4, 4)]), (8, 48): ([(8, 8)], [(8, 8)]),
+                   (16, 16): ([(4, 8), (8, 4), (4, 16), (16, 4), (4, 32), (32, 4), (4, 64), (64, 4)], [(4, 8), (16, 4)]),
+                   (16, 48): ([(16, 16), (8, 16), (16, 8), (32, 32), (64, 64), (8, 64), (64, 16)], [(16, 16), (32, 32), (8, 32)])}
+
+
+def k1_tr_sides(n):
+    """The 1-D transforms a side of n samples can take: DST-7 and DCT-8 exist for 4..32."""
+    return (abi.TR_DCT2, abi.TR_DST7, abi.TR_DCT8) if 4 <= n <= 32 else (abi.TR_DCT2,)
+
+
+def k1_zero_out(tr, n):
+    """How many coefficients of a side can be coded: 16 for DST-7 / DCT-8 at 32, else min(n, 32)."""
+    return 16 if tr != abi.TR_DCT2 and n == 32 else min(n, 32)
+
+
+def k1_lfnst_form(w, h):
+    """(zeroOutSize, outputs) of LFNST on a w x h block: 8 inputs on 4x4 and 8x8, 48 outputs when both sides are at least 8."""
+    return (8 if (w, h) in ((4, 4), (8, 8)) else 16), (48 if w >= 8 and h >= 8 else 16)
+
+
+class _K1Case:
+    """TU records packed row by row into their planes (luma; one shelf for both chroma planes, so a joint-CbCr partner never overlaps another TU)."""
+    def __init__(self, W, bd, rng):
+        self.W, self.bd, self.rng = W, bd, rng
+        self.recs, self.levels, self.tags, self.syntax, self.n = [], [], [], [], 0
+        self.shelf = [[0, 0, 0], [0, 0, 0]]
+
+    def place(self, comp, w, h):
+        s, pw = self.shelf[comp > 0], self.W >> (comp > 0)
+        if s[0] + w > pw: s[0], s[1], s[2] = 0, s[1] + s[2], 0
+        x, y = s[0], s[1]
+        s[0] += w; s[2] = max(s[2], h)
+        return x, y
+
+    def height(self):
+        return max(8, self.shelf[0][1] + self.shelf[0][2], 2 * (self.shelf[1][1] + self.shelf[1][2]) + 8) + 7 & ~7
+
+    def add(self, tag, comp, w, h, lv, qp, dq=False, tr=0, lfnst=0, ict=0, flags=0, sl_off=0, syntax=None, at=None, dqp=None):
+        """qp = QP (QP' - 6 (bd - 8)); lv = the level corner (rows maxY + 1, columns maxX + 1).  A chroma TU with a syntax form keeps qp <= 26, where the
+        default chroma QP mapping is the identity."""
+        lv = np.asarray(lv, np.int16).reshape(np.shape(lv)[0], -1)
+        l2w, l2h = w.bit_length() - 1, h.bit_length() - 1
+        x, y = at or self.place(comp, w, h)
+        rs, ib, sc = dqp or tu_dequant(qp + 6 * (self.bd - 8), self.bd, l2w, l2h, bool(flags & abi.TU_TS), dq, bool(flags & abi.TU_SCALING))
+        self.recs.append((x, y, l2w, l2h, comp, flags, lv.shape[1] - 1, lv.shape[0] - 1, tr, lfnst, ict, rs, ib, sc, self.n, sl_off, (0, 0)))
+        self.levels.append(lv.reshape(-1)); self.n += lv.size; self.tags.append(tag)
+        self.syntax.append(None if syntax is None else dict(syntax, comp=comp, bitDepth=self.bd, qp=qp, depQuant=int(dq),
+                                                            w=w << (comp > 0), h=h << (comp > 0)))
+
+    def extreme(self, k, rows, cols):
+        """Saturating levels whose signs follow a basis row: all +32767 / all -32768 (row 0 of DCT-2, DST-7 and DCT-8 has one sign), signs alternating
+        by coefficient row or column (the last DCT-2 row), or a random sign per level."""
+        yy, xx = np.mgrid[0:rows, 0:cols]
+        sign = [np.ones_like(yy), -np.ones_like(yy), 1 - 2 * (yy & 1), 1 - 2 * (xx & 1), self.rng.choice([-1, 1], size=(rows, cols))][k % 5]
+        return np.where(sign > 0, 32767, -32768)
+
+
+def _k1_pair_syntax(w, h, trH, trV):
+    """A luma syntax form that selects (trH, trV) on a w x h TU: DCT-2 on an inter CU, explicit MTS, or implicit MTS (DST-7 on sides 4..16 of an intra
+    CU of at most 32x32, DCT-2 on the others); None where only SBT / ISP give the pair."""
+    D2, S7, C8 = abi.TR_DCT2, abi.TR_DST7, abi.TR_DCT8
+    if trH == D2 and trV == D2: return dict(predMode=0)
+    if trH != D2 and trV != D2: return dict(predMode=1, spsMTS=1, spsIntraMTS=1, mtsIdx=2 + (trH == C8) + 2 * (trV == C8))
+    if max(w, h) <= 32 and (trH == S7) == (w <= 16) and (trV == S7) == (h <= 16) and C8 not in (trH, trV):
+        return dict(predMode=1, spsMTS=1, spsIntraMTS=0)
+    return None
+
+
+def _k1_pairs(b):
+    """Every shape x every legal (trH, trV): DC only, the whole zero-out corner (random and saturating levels) and an odd corner."""
+    k = 0
+    for l2w in range(1, 7):
+        for l2h in range(1, 7):
+            w, h = 1 << l2w, 1 << l2h
+            comp = 0 if min(w, h) >= 4 else 1 + (k & 1)                 # sides of 2 only exist in chroma
+            for trH in k1_tr_sides(w):
+                for trV in k1_tr_sides(h):
+                    tr, zx, zy = trH | (trV << 2), k1_zero_out(trH, w), k1_zero_out(trV, h)
+                    ox, oy = [v for v in K1_ODD if v <= zx], [v for v in K1_ODD if v <= zy]
+                    ox, oy = ox[k % len(ox)], oy[(k // len(ox)) % len(oy)]
+                    syn = _k1_pair_syntax(w, h, trH, trV) if comp == 0 else None
+                    tag = f"pairs {w}x{h} {K1_TR_NAMES[trH]}x{K1_TR_NAMES[trV]}"
+                    b.add(tag + " DC only", comp, w, h, [[int(b.rng.integers(1, 3000)) * (1 - 2 * (k & 1))]], 30, tr=tr, syntax=syn)
+                    b.add(tag + " full", comp, w, h, b.rng.integers(-300, 301, (zy, zx)), 27, dq=bool(k & 1), tr=tr, syntax=syn)
+                    b.add(tag + " full saturating", comp, w, h, b.extreme(k, zy, zx), 37, tr=tr, syntax=syn)
+                    b.add(tag + f" odd corner {ox}x{oy}", comp, w, h, b.rng.integers(-300, 301, (oy, ox)), 32, tr=tr, syntax=syn)
+                    k += 1
+
+
+def _k1_lfnst(b):
+    """Every (set, index, transpose) x every LFNST form x one-hot input at each of the 16 scan positions (corner 4x4 or just reaching the input), and all
+    16 inputs saturated."""
+    i = 0
+    for form, (luma, chroma) in K1_LFNST_SHAPES.items():
+        shapes = [(0, s) for s in luma] + [(1, s) for s in chroma]
+        for (st, tp), mode in K1_LFNST_MODES.items():
+            for idx in (1, 2):
+                code = idx | (st << 2) | (tp << 4)
+                for pos in range(17):
+                    comp, (w, h) = shapes[i % len(shapes)]
+                    comp = comp and 1 + (i & 1)
+                    i += 1
+                    if pos < 16:
+                        y, x = K1_SCAN[pos]
+                        lv = np.zeros((4, 4) if i & 1 else (y + 1, x + 1), np.int16)
+                        lv[y, x] = int(b.rng.integers(50, 600)) * (1 - 2 * (pos & 1))
+                        tag = f"lfnst set {st} idx {idx} transpose {tp} {w}x{h} input {pos}"
+                    else:
+                        lv, tag = b.extreme(i, 4, 4), f"lfnst set {st} idx {idx} transpose {tp} {w}x{h} all 16 inputs saturated"
+                    pinned = w == h and (pos < form[0] or pos == 16)          # the parser never codes inputs past zeroOutSize
+                    syn = dict(predMode=1, spsLFNST=1, lfnstIdx=idx, sepTree=int(comp > 0), intraDirL=mode, intraDirC=mode) if pinned else None
+                    b.add(tag, comp, w, h, lv, 22 if pos < 16 else 26, lfnst=code, syntax=syn)
+
+
+def _k1_dequant(b):
+    """Every QP of the bit depth, with and without dependent quantisation, on 4x4 / 8x4 luma (all 12 scales) and 2x4 / 2x2 chroma (the most negative
+    shifts): levels at +-inMax, +-(inMax + 1) and +-32768 through transform skip (the residual is the dequantised level), DC-only DCT-2 and full corners;
+    every third QP also with a scaling list of entries 1 and 255; 2x2 records with shifts of -10..-12 and every scale, where the inMax clip binds."""
+    bd = b.bd
+    for qp in range(-6 * (bd - 8), 64):
+        for dq in (False, True):
+            for comp, w, h, kind in ((0, 4, 4, "ts"), (0, 4, 4, "dc"), (0, 8, 4, "dc"), (0, 4, 4, "full"), (1, 2, 4, "full"), (2, 2, 2, "full")):
+                ts = kind == "ts"
+                if ts and dq: continue
+                rs, ib, _ = tu_dequant(qp + 6 * (bd - 8), bd, w.bit_length() - 1, h.bit_length() - 1, ts, dq)
+                m = (1 << (ib - 1)) - 1
+                vals = np.array([m, -m, min(m + 1, 32767), -m - 1, 32767, -32768, 1, -1], np.int64)
+                lv = np.array([[vals[(qp + dq) % len(vals)]]]) if kind == "dc" else b.rng.choice(vals, size=(h, w))
+                syn = dict(predMode=0, mtsIdx=int(ts)) if comp == 0 or (h == 4 and qp <= 26) else None
+                tag = f"dequant QP {qp}{' depquant' if dq else ''} {w}x{h} {kind} rightShift {rs}"
+                b.add(tag, comp, w, h, lv, qp, dq=dq, flags=abi.TU_TS if ts else 0, syntax=syn)
+                if qp % 3 == 0 and comp == 0 and not ts:
+                    b.add(tag + " scaling list 1 / 255", comp, w, h, lv, qp, dq=dq, flags=abi.TU_SCALING, sl_off=b.sl_off[(w, h)])
+    # the inMax clip keeps level * scale << -rightShift inside 32 bits: shifts past the decoder's, with every scale (records only)
+    for rs in (-10, -11, -12):
+        for sc in sorted({s for row in TU_INV_SCALES for s in row}):
+            lv = b.rng.choice([32767, -32768, 1 << (24 + rs), -(1 << (24 + rs)) - 1], size=(2, 2))
+            b.add(f"dequant rightShift {rs} scale {sc}", 2, 2, 2, lv, 0, dqp=(rs, min(16, 25 + rs), sc))
+
+
+def _k1_ts_bdpcm(b):
+    """Transform skip at every size up to 32 (2xN / Nx2 chroma included), and BDPCM H and V whose lines of +32767 / -32768 saturate the running sum."""
+    shapes = [(0, w, h) for w in (4, 8, 16, 32) for h in (4, 8, 16, 32)] + [(1, w, h) for w in (2, 4, 8, 16) for h in (2, 4, 8, 16)]
+    for k, (comp, w, h) in enumerate(shapes):
+        comp = comp and 1 + (k & 1)
+        qp = 4 - 6 * (b.bd - 8)                                         # QP' 4: the dequantised level is the level
+        syn = dict(predMode=0, mtsIdx=1)
+        b.add(f"ts {w}x{h}", comp, w, h, b.rng.integers(-32768, 32768, (h, w)), qp, flags=abi.TU_TS, syntax=syn)
+        b.add(f"ts {w}x{h} QP 25", comp, w, h, b.rng.integers(-400, 401, (h, w)), 25, flags=abi.TU_TS, syntax=syn)
+        for mode, flag in ((1, abi.TU_BDPCM_H), (2, abi.TU_BDPCM_V)):
+            n, length = (h, w) if mode == 1 else (w, h)
+            lines = [np.full(length, 32767), np.full(length, -32768), np.where(np.arange(length) & 1, -32768, 32767),
+                     np.where(np.arange(length) < length // 2, 32767, -32768), b.rng.integers(-20000, 20001, length)]
+            lv = np.array([lines[(i + k) % len(lines)] for i in range(n)])
+            lv = lv if mode == 1 else lv.T
+            syn = dict(predMode=1, mtsIdx=1, **({"bdpcmL": mode} if comp == 0 else {"bdpcmC": mode}))
+            for q in (qp, 25):
+                b.add(f"bdpcm {'HV'[mode - 1]} {w}x{h} QP {q}", comp, w, h, lv, q, flags=abi.TU_TS | flag, syntax=syn)
+
+
+def _k1_jccr(b):
+    """Joint CbCr: every ict on Cb and on Cr, with residuals -32768, -1, +1, odd negatives and +32767 (transform skip at QP' 4) and transform blocks of
+    saturating and random levels; run on predictions of 0 and pmax."""
+    vals = np.array([-32768, -1, 1, -3, -5, -32767, 32767, 3, -7, 0], np.int64)
+    k = 0
+    for comp in (1, 2):
+        for ict in (1, -1, 2, -2, 3, -3):
+            for w, h in ((2, 2), (2, 4), (4, 2), (4, 4), (8, 8), (16, 16), (32, 32), (8, 2)):
+                syn = dict(jointCbCr={1: 2, 2: 3, 3: 1}[abs(ict)], jointCbCrSign=int(ict < 0)) if (abs(ict) == 3) == (comp == 2) and (w, h) != (2, 2) else None
+                tag = f"jccr ict {ict} comp {comp} {w}x{h}"
+                b.add(tag + " ts", comp, w, h, b.rng.choice(vals, size=(h, w)), 4 - 6 * (b.bd - 8), ict=ict, flags=abi.TU_TS,
+                      syntax=syn and dict(syn, predMode=0, mtsIdx=1))
+                zx, zy = min(w, 32), min(h, 32)
+                b.add(tag + " saturating", comp, w, h, b.extreme(k, zy, zx), 26, ict=ict, syntax=syn and dict(syn, predMode=0))
+                b.add(tag + " random", comp, w, h, b.rng.integers(-900, 901, (zy, zx)), 24, ict=ict, dq=True, syntax=syn and dict(syn, predMode=0))
+                k += 1
+
+
+# name -> (kind, bit depth, width, height (None: as packed), 4:2:0?, strides or None, prediction)
+K1_SWEEP_CASES = {
+    "pairs_10bit": ("pairs", 10, 1024, None, True, (1029, 515, 517), "noise"),
+    "lfnst_10bit": ("lfnst", 10, 1024, None, True, (1032, 516, 516), "noise"),
+    "dequant_8bit": ("dequant", 8, 256, None, True, (260, 131, 130), "noise"),
+    "dequant_9bit": ("dequant", 9, 256, None, True, None, "noise"),
+    "dequant_10bit": ("dequant", 10, 256, None, True, (257, 128, 129), "noise"),
+    "dequant_12bit": ("dequant", 12, 256, None, True, None, "extreme"),
+    "ts_bdpcm_10bit": ("ts_bdpcm", 10, 512, None, True, (515, 257, 259), "noise"),
+    "ts_bdpcm_8bit": ("ts_bdpcm", 8, 512, None, True, None, "extreme"),
+    "jccr_10bit": ("jccr", 10, 512, None, True, (516, 259, 258), "extreme"),
+    "jccr_12bit": ("jccr", 12, 512, None, True, None, "extreme"),
+    "geometry_400": ("random", 10, 256, 136, False, (261, 0, 0), "noise"),
+    "geometry_9bit_odd_strides": ("random", 9, 200, 136, True, (203, 101, 107), "noise"),
+    "geometry_12bit_edges": ("random", 12, 392, 264, True, None, "extreme"),
+    "uhd_3840x2160": ("random", 10, 3840, 2160, True, None, "noise"),
+}
+
+
+def _k1_case(name):
+    import zlib
+    kind, bd, W, H, chroma, strides, pred = K1_SWEEP_CASES[name]
+    rng = np.random.default_rng(zlib.crc32(name.encode()))
+    scaling = None
+    if kind == "random":
+        # dense TUs of every kind over a whole partitioned picture: its last row and column included
+        cus = partition(rng, W, H, ctu=128)
+        tus, coefs = gen_tus(rng, cus, bd, p_cbf=0.9, p_mts=0.25, p_lfnst=0.2, p_ts=0.15, p_bdpcm=0.1, p_jccr=0.3, p_full=0.8, chroma=chroma,
+                             heavy=0.3, p_intra=0.6)
+        tags, syntax = ["geometry"] * len(tus), [None] * len(tus)
+    else:
+        b = _K1Case(W, bd, rng)
+        if kind == "dequant":
+            b.sl_off = {(4, 4): 0, (8, 4): 16}
+            scaling = np.where((np.arange(48) + np.arange(48) // 4) & 1, 255, 1).astype(np.int32)
+        {"pairs": _k1_pairs, "lfnst": _k1_lfnst, "dequant": _k1_dequant, "ts_bdpcm": _k1_ts_bdpcm, "jccr": _k1_jccr}[kind](b)
+        H = b.height()
+        tus, coefs, tags, syntax = np.array(b.recs, abi.TU_DTYPE), np.concatenate(b.levels), b.tags, b.syntax
+    pmax = (1 << bd) - 1
+
+    def content(c, w, h):
+        if pred == "noise": return noise_planes(rng, w, h, bd, chroma=False)[0]
+        yy, xx = np.mgrid[0:h, 0:w]                                     # 4x4 blocks of 0 and pmax, Cr the inverse of Cb
+        return np.where(((yy >> 2) + (xx >> 2) + (c == 2)) & 1, pmax, 0)
+    planes = _k45_planes(W, H, chroma, strides, content)
+    if not chroma: planes += [None, None]
+    g = abi.make_geom(W, H, bd, chroma_format=1 if chroma else 0, strides=strides)
+    return dict(name=name, kind=kind, g=g, W=W, H=H, bd=bd, chroma=chroma, strides=strides, planes=planes, tus=tus, coefs=coefs, scaling=scaling,
+                tags=tags, syntax=syntax)
+
+
+_k1_cache = {}
+
+
+def k1_sweep(name):
+    """One case of the designed K1 sweep (K1_SWEEP_CASES): geometry (g, W, H, bd, chroma, strides), prediction planes (stride padding holds -7; None for
+    absent chroma), TU records, level arena, scaling arena (or None), per-TU tags and syntax (None: a record only the record interface allows).
+    pairs: every shape x (trH, trV) with DC-only, zero-out and odd corners and saturating levels; lfnst: every set / index / transpose x LFNST form x
+    input position; dequant: every QP, both quantisers, all scales, the most negative shifts, inMax and scaling-list extremes; ts_bdpcm: transform skip
+    at every size and saturating BDPCM lines; jccr: every ict on both chroma planes over 0 / pmax predictions; geometry: 4:0:0, odd strides, picture
+    edges, 4K."""
+    if name not in _k1_cache: _k1_cache[name] = _k1_case(name)
+    c = _k1_cache[name]
+    return dict(c, planes=[None if p is None else p.copy() for p in c["planes"]])
+
+
+def k1_corner(tus, coefs, i):
+    """The level corner of TU i: (maxY + 1, maxX + 1) int16."""
+    t = tus[i]
+    mx, my, off = int(t["maxX"]) + 1, int(t["maxY"]) + 1, int(t["coefOff"])
+    return coefs[off:off + mx * my].reshape(my, mx)
+
+
+def k1_lmcs_picture(ctu, W=256, H=128, bd=10):
+    """TUs and prediction for LMCS chroma residual scaling on the picture path: luma constant per VPDU, at values spread over the LMCS bins, so that the
+    VPDUs' neighbourhoods pick different chromaAdjHelpLUT entries; in each VPDU's chroma area a 2x2 TU (never scaled), 2x4 and 4x2 TUs, 4x4 / 8x8 TUs and
+    joint-CbCr pairs (transform skip with the level as residual, and DCT-2), and one luma TU.  Returns (tus, coefs, given planes, tags)."""
+    import zlib
+    rng = np.random.default_rng(zlib.crc32(f"lmcs{ctu}".encode()))
+    b = _K1Case(W, bd, rng)
+    vs = 64 if ctu == 128 else ctu
+    pmax = (1 << bd) - 1
+    luma = np.zeros((H, W), np.int16)
+    ts = dict(flags=abi.TU_TS, qp=4 - 6 * (bd - 8))
+    for k, (vy, vx) in enumerate((vy, vx) for vy in range(0, H, vs) for vx in range(0, W, vs)):
+        luma[vy:vy + vs, vx:vx + vs] = 24 + ((k * 7) % 16) * ((pmax - 48) // 15)
+        cx, cy, ict = vx // 2, vy // 2, (1, -1, 2, -2, 3, -3)[k % 6]
+        for comp, w, h, dx, dy, kw in ((1, 2, 2, 0, 0, ts), (2, 2, 4, 2, 0, ts), (1, 4, 2, 4, 0, ts), (1 + (abs(ict) == 3), 4, 4, 8, 0, dict(ts, ict=ict)),
+                                        (2, 4, 4, 12, 0, dict(qp=27)), (1 + (abs(ict) == 3), 8, 8, 0, 8, dict(qp=24, ict=-ict)), (1, 8, 8, 8, 8, ts)):
+            lv = rng.integers(-300, 301, (h, w))
+            b.add(f"lmcs VPDU {k} comp {comp} {w}x{h}{' ict %d' % kw['ict'] if 'ict' in kw else ''}", comp, w, h, lv, at=(cx + dx, cy + dy), **kw)
+        b.add(f"lmcs VPDU {k} luma 8x8", 0, 8, 8, rng.integers(-40, 41, (8, 8)), 30, at=(vx + 8, vy + 8))
+    chroma = [(pmax // 2 + rng.integers(-100, 101, (H // 2, W // 2))).astype(np.int16) for _ in range(2)]
+    return np.array(b.recs, abi.TU_DTYPE), np.concatenate(b.levels), [luma] + chroma, b.tags
