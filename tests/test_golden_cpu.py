@@ -115,6 +115,18 @@ def test_chain_golden(oracle):
     for c in range(3): assert np.array_equal(out[c], z[f"out{c}"]), f"plane {c}"
 
 
+def test_lmcs_golden(oracle):
+    """tests/golden/lmcs_pictures.npz: LMCS sweep pictures at 8 and 12 bit (designed VPDU neighbourhoods, scaled chroma TUs) through the reference arm."""
+    from tests.helpers import oracle_decompress
+    z = _load("lmcs_pictures.npz")
+    assert len(z["names"]) == 2
+    for name in [str(n) for n in z["names"]]:
+        c = synth.lmcs_sweep(name)
+        assert np.array_equal(c["pic"]["given"][0], z[f"{name}_given0"]), name     # the sweep still builds the fixture's input
+        out, _ = oracle_decompress(oracle, c["g"], c["dpb"], c["pic"])
+        for k in range(3): assert np.array_equal(out[k], z[f"{name}_out{k}"]), (name, k)
+
+
 def test_film_grain_golden(oracle):
     """tests/golden/film_grain_fgc.npz: tables from the reference's FGC firmware, output of its SIMD line kernels (third frame of a sequence)."""
     z = _load("film_grain_fgc.npz")

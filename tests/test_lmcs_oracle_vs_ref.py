@@ -74,6 +74,67 @@ def test_vpdu_chroma_scale(oracle, ref, ctu, W, H):
             assert got == want, (vx, vy)
 
 
+def build_model(ref, name, bd):
+    """designed model -> (Lmcs from the REAL constructReshaper, its invLUT, the generator's dict)"""
+    m = synth.lmcs_model(name, bd)
+    L = abi.Lmcs(); lut = np.zeros(1 << bd, np.int16)
+    assert ref.ref_lmcs_build(bd, m["minBin"], m["maxBin"], (C.c_int * 16)(*m["delta"]), m["chrOff"], 1, C.byref(L), lut) == 0, name
+    return L, lut, m
+
+
+@pytest.mark.parametrize("bd", [8, 10, 12])
+def test_designed_models_match_construct_reshaper(oracle, ref, bd):
+    """Every designed model (synth.LMCS_MODELS): constructReshaper accepts it and builds lmcs_tables' tables; rspBufFwd / applyLut on a ramp of every
+    value equal the oracle's forward map and the LUT (scalar and SIMD).  The SIMD inverse (rspBcw, piece-wise linear) agrees with the LUT on every
+    designed model."""
+    n = 1 << bd
+    for name in synth.LMCS_MODELS:
+        L, lut, m = build_model(ref, name, bd)
+        G = m["struct"]
+        assert (L.orgCW, L.minBinIdx, L.maxBinIdx) == (G.orgCW, G.minBinIdx, G.maxBinIdx), name
+        assert list(L.reshapePivot) == list(G.reshapePivot) and list(L.inputPivot) == list(G.inputPivot), name
+        assert list(L.fwdScaleCoef) == list(G.fwdScaleCoef) and list(L.chromaAdjHelpLUT) == list(G.chromaAdjHelpLUT), name
+        assert np.array_equal(lut, m["invLUT"]), name
+        st = 64
+        ramp = np.arange(((n + st - 1) // st) * st).reshape(-1, st).astype(np.int16) % n
+        for simd in (0, 1):
+            a = aligned_copy(ramp); b = aligned_copy(ramp)
+            ref.ref_lmcs_fwd_block(simd, a.ctypes.data, st, st, len(ramp))
+            oracle.orc_lmcs_fwd_block(b.ctypes.data, st, st, len(ramp), bd, C.byref(L))
+            assert np.array_equal(a, b), ("fwd", name, simd)
+            a = aligned_copy(ramp)
+            ref.ref_lmcs_inv_block(simd, a.ctypes.data, st, st, len(ramp))
+            assert np.array_equal(a, lut[ramp]), ("inv", name, simd, int((a != lut[ramp]).sum()))
+
+
+@pytest.mark.parametrize("bd", [8, 10, 12])
+def test_designed_vpdu_neighbourhoods(oracle, ref, bd):
+    """calculateChromaAdjVpduNei on the sweep's designed neighbourhoods (one CU per CTU at CTU 32 and 64, as the shim's structure; averages on every
+    pivot, walks clamped at the picture's last row / column) equals orc_lmcs_vpdu_scale for every VPDU."""
+    for var in ("ctu32", "ctu64"):
+        name = [k for k in synth.LMCS_SWEEP if k.startswith("vpdu_") and k.endswith(f"_{bd}bit_{var}")][0]
+        c = synth.lmcs_sweep(name)
+        m = c["pic"]["lmcs"]
+        L, lut, _ = build_model(ref, m["name"], bd)
+        vs = min(64, c["ctu"]); vW = (c["W"] + vs - 1) // vs
+        planes = [c["pic"]["given"][0], np.zeros((c["H"] // 2, c["W"] // 2), np.int16), np.zeros((c["H"] // 2, c["W"] // 2), np.int16)]
+        for i, v in enumerate(m["vpdus"]):
+            want = ref.ref_lmcs_vpdu_scale(C.byref(c["g"]), abi.plane_ptrs(planes), (i % vW) * vs, (i // vW) * vs)
+            vv = abi.LmcsVpdu(int(v["x"]), int(v["y"]), int(v["availLeft"]), int(v["availAbove"]))
+            assert oracle.orc_lmcs_vpdu_scale(C.byref(c["g"]), planes[0], C.byref(m["struct"]), C.byref(vv)) == want, (name, i)
+
+
+@pytest.mark.parametrize("name", ["vpdu_full_bins_8bit_ctu32", "vpdu_full_bins_10bit_ctu32", "vpdu_full_bins_12bit_ctu32", "extremes_crs_min_12bit"])
+def test_sweep_pictures_reference_arm(oracle, ref, name):
+    """The reference arm (ref_decompress_picture_out, SIMD off) equals oracle_decompress on sweep pictures whose records are CTU origins."""
+    c = synth.lmcs_sweep(name)
+    want, _ = oracle_decompress(oracle, c["g"], c["dpb"], c["pic"])
+    got = [np.zeros_like(p) for p in want]
+    ref.ref_decompress_picture_out(C.byref(c["g"]), ref_ptrs(c["dpb"]), C.byref(c["pic"]["struct"]), 2, 0, abi.plane_ptrs(got))
+    for k in range(3):
+        assert np.array_equal(want[k], got[k]), (name, k, int((want[k] != got[k]).sum()))
+
+
 @pytest.mark.parametrize("simd", [0, 1])
 @pytest.mark.parametrize("chroma_adj", [True, False])
 def test_picture_with_lmcs(oracle, ref, simd, chroma_adj):

@@ -141,8 +141,23 @@ def intra():
                         **{f"resi{c}": resi[c] for c in range(3)}, **{f"out{c}": out[c] for c in range(3)})
 
 
+def lmcs():
+    """LMCS sweep pictures (synth.lmcs_sweep: designed VPDU neighbour averages on every pivot of full_bins, DC / 4-sample / joint-CbCr chroma TUs) at 8
+    and 12 bit through the reference arm (its own calculateChromaAdjVpduNei / scaleSignal / applyLut, SIMD off).  The sweep's records are CTU origins at
+    CTU 32, the reference arm's one CU per CTU.  The inputs are rebuilt from the sweep; the fixture keeps the `given` luma as a check of that."""
+    names = ["vpdu_full_bins_8bit_ctu32", "vpdu_full_bins_12bit_ctu32"]
+    out = dict(names=np.array(names))
+    for name in names:
+        c = synth.lmcs_sweep(name)
+        o = [np.zeros((c["H"], c["W"]), np.int16), np.zeros((c["H"] // 2, c["W"] // 2), np.int16), np.zeros((c["H"] // 2, c["W"] // 2), np.int16)]
+        ref.ref_decompress_picture_out(C.byref(c["g"]), ref_ptrs(c["dpb"]), C.byref(c["pic"]["struct"]), 2, 0, abi.plane_ptrs(o))
+        out[f"{name}_given0"] = c["pic"]["given"][0]
+        out.update({f"{name}_out{k}": o[k] for k in range(3)})
+    np.savez_compressed(os.path.join(OUT, "lmcs_pictures.npz"), **out)
+
+
 if __name__ == "__main__":
     import sys
     if len(sys.argv) > 1: [globals()[n]() for n in sys.argv[1:]]
-    else: k1(); pictures(); chain(); film_grain(); intra()
+    else: k1(); pictures(); chain(); film_grain(); intra(); lmcs()
     print({f: os.path.getsize(os.path.join(OUT, f)) for f in sorted(os.listdir(OUT))})

@@ -159,6 +159,7 @@ int k1_launch_count(const K1Launch& L);
 struct LmcsLaunch { b200_geom geom; DevPlanes planes; const b200_lmcs* lmcs; const b200_lmcs_vpdu* vpdus; const int16_t* invLut; int* scale; };
 int launch_lmcs_vpdu(const LmcsLaunch& L, cudaStream_t s);   // per-VPDU chroma residual scale from the reconstructed (mapped) luma
 int launch_lmcs_inv(const LmcsLaunch& L, cudaStream_t s);    // inverse map of the luma plane, in place
+int launch_lmcs_validate(const b200_lmcs_vpdu* vpdus, const b200_geom& g, int* meta, cudaStream_t s);   // after launch_mc_bucket (same meta block)
 
 int launch_pack(const DevPlanes& src, const b200_geom& g, int fmt, uint8_t* const dst[3], cudaStream_t s);   // output.cu: pyuv / 8-bit conversion
 

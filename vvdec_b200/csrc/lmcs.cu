@@ -55,6 +55,22 @@ __global__ void __launch_bounds__(256) lmcs_inv_kernel(int16_t* __restrict__ lum
   }
 }
 
+// every VPDU record against lmcs_vpdu_problem (rules.cuh): error bit 16 of the PU meta block, read by b200_pic_run before lmcs_vpdu_kernel runs
+__global__ void __launch_bounds__(256) lmcs_validate_kernel(const b200_lmcs_vpdu* __restrict__ vpdus, int numVpdus, const b200_geom g, int* meta)
+{
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i < numVpdus && lmcs_vpdu_problem(vpdus[i], i, g)) atomicOr(&meta[LM_ERR], 16);
+}
+
+int launch_lmcs_validate(const b200_lmcs_vpdu* vpdus, const b200_geom& g, int* meta, cudaStream_t s)
+{
+  const int vs = g.ctuSize == 128 ? 64 : g.ctuSize;
+  const int n = ((g.width + vs - 1) / vs) * ((g.height + vs - 1) / vs);
+  lmcs_validate_kernel<<<(n + 255) / 256, 256, 0, s>>>(vpdus, n, g, meta);
+  B200_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int launch_lmcs_vpdu(const LmcsLaunch& L, cudaStream_t s)
 {
   const int vs = L.geom.ctuSize == 128 ? 64 : L.geom.ctuSize;

@@ -150,7 +150,8 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   if (why) { set_error("b200_pic_upload: %s", why); return B200_ERR_PARAM; }
   B200_CHECK(p->numPus < (1u << 26) && p->numTus < (1u << 31), "b200_pic_upload: too many records");
   B200_CHECK(p->numWp >= 0 && p->numWp <= 255 && (p->wp || !p->numWp), "b200_pic_upload: weighted-prediction table (at most 255 entries)");
-  B200_CHECK(!(p->flags & B200_PIC_LMCS) || (p->lmcs && p->lmcs->invLUT && (!p->lmcs->chromaAdj || p->lmcs->vpdus) && p->lmcs->orgCW == (1 << c->g.bitDepth) / 16), "b200_pic_upload: LMCS data missing or inconsistent");
+  B200_CHECK(!(p->flags & B200_PIC_LMCS) || (p->lmcs && p->lmcs->invLUT && (!p->lmcs->chromaAdj || p->lmcs->vpdus)), "b200_pic_upload: LMCS data missing");
+  if (p->flags & B200_PIC_LMCS) if (const char* why = lmcs_model_problem(*p->lmcs, c->g.bitDepth)) { set_error("b200_pic_upload: %s", why); return B200_ERR_PARAM; }
   B200_CHECK(!p->numIntraTus || (p->intraTus && p->numIntraTus < (1u << 30)), "b200_pic_upload: intra list missing");
   B200_CUDA(cudaSetDevice(c->device));
   const int ai = c->nextArena; c->nextArena = (c->nextArena + 1) % c->numArenas;
@@ -260,6 +261,7 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
     if (any) c->launches += 1;
   }
   if (A.numIntraTus) { if (int rc = launch_intra_validate(A.intraTus, A.numIntraTus, g, A.mcMeta, s)) return rc; c->launches += 1; }
+  if (A.lmcsChromaAdj) { if (int rc = launch_lmcs_validate(A.lmcsVpdus, g, A.mcMeta, s)) return rc; c->launches += 1; }
   B200_CUDA(cudaMemcpyAsync(A.hMeta, A.mcMeta, 2 * LM_INTS * sizeof(int), cudaMemcpyDeviceToHost, s));   // list lengths for b200_pic_run's grids
   B200_CUDA(cudaEventRecord(A.uploaded, s));
   return ai;
@@ -278,6 +280,7 @@ B200_API int b200_pic_run(b200_ctx* c, int ai)
   B200_CHECK(!(A.hMeta[LM_ERR] & 2), "b200_pic_run: more MC tiles than the picture can hold (overlapping PUs?)");
   B200_CHECK(!(A.hMeta[LM_ERR] & 8), "b200_pic_run: an intra block record is invalid (geometry, mode, or availability reaching outside the picture)");
   B200_CHECK(!(A.hMeta[LM_ERR] & 4), "b200_pic_run: a CTU record (SAO type / band, ALF filter index or clip / pad flags, slice index) is out of range");
+  B200_CHECK(!(A.hMeta[LM_ERR] & 16), "b200_pic_run: an LMCS VPDU record is invalid (CU origin outside the picture or not at or above-left of its VPDU in the same CTU, or an available neighbour outside the picture)");
   B200_CHECK(!A.hMeta[LM_INTS + LM_ERR], "b200_pic_run: the picture's TU list holds an invalid record");
   B200_CUDA(cudaStreamWaitEvent(s, A.uploaded, 0));
   const b200_geom& g = c->g;

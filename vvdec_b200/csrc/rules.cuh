@@ -1,6 +1,6 @@
 // rules.cuh — what a geometry and every kind of record must satisfy before a kernel may use it, stated once.  The kernel-level wrappers (api.cu) check
 // each record on the host with these functions before any device work; the picture path (picture.cu) checks its O(1) inputs on the host and its
-// records on the device (bucket.cu, k6_intra.cu), where a failure raises one error bit per list.  Each function returns nullptr for a legal input, or
+// records on the device (bucket.cu, k6_intra.cu, lmcs.cu), where a failure raises one error bit per list.  Each function returns nullptr for a legal input, or
 // a short reason: the host prints it after the entry point's name, the device only tests it for null.
 #pragma once
 #include <stdint.h>
@@ -178,6 +178,32 @@ inline CtuLimits ctu_limits(const b200_geom& g, const b200_alf_tables* T, int nu
   l.numLumaSets = T ? T->numLumaSets : 0; l.numChromaAlts = T ? T->numChromaAlts : 0; l.numCc[0] = T ? T->numCc[0] : 0; l.numCc[1] = T ? T->numCc[1] : 0;
   l.numLfSlices = numLfSlices; l.ctusW = (g.width + g.ctuSize - 1) / g.ctuSize; l.ctusH = (g.height + g.ctuSize - 1) / g.ctuSize;
   return l;
+}
+
+// ---- LMCS: the model (b200_lmcs) and the per-VPDU records (b200_lmcs_vpdu) ----
+// lmcs_vpdu_kernel walks reshapePivot[minBinIdx + 1 .. maxBinIdx + 1]; the pivots and input pivots are the ones constructReshaper (reference
+// CommonLib/Reshape.cpp:317) builds from a legal APS: LmcsPivot[0] = 0, non-decreasing up to at most 2^bitDepth, InputPivot[i] = i * OrgCW
+__host__ __device__ inline const char* lmcs_model_problem(const b200_lmcs& L, int bitDepth)
+{
+  const int org = (1 << bitDepth) / 16;
+  if (L.orgCW != org) return "LMCS model: orgCW is not (1 << bitDepth) / 16";
+  if (L.minBinIdx < 0 || L.minBinIdx > L.maxBinIdx || L.maxBinIdx > 15) return "LMCS model: bins (0 <= minBinIdx <= maxBinIdx <= 15)";
+  if (L.reshapePivot[0] != 0) return "LMCS model: reshapePivot[0] is not 0";
+  for (int i = 0; i < 16; i++) if (L.reshapePivot[i + 1] < L.reshapePivot[i]) return "LMCS model: reshapePivot decreases";
+  if (L.reshapePivot[16] > (1 << bitDepth)) return "LMCS model: reshapePivot[16] above 2^bitDepth";
+  for (int i = 0; i < 17; i++) if (L.inputPivot[i] != i * org) return "LMCS model: inputPivot[i] is not i * orgCW";
+  return nullptr;
+}
+// record i of the raster of VPDUs (64x64, or the CTU when it is smaller): the CU that covers the VPDU's top-left sample starts at or above-left of it
+// in the same CTU, and a neighbour is available only where it lies inside the picture.  lmcs_vpdu_kernel then reads column x - 1 and row y - 1 of the
+// luma plane, clamped to its last row / column, and nothing else.
+__host__ __device__ inline const char* lmcs_vpdu_problem(const b200_lmcs_vpdu& v, int i, const b200_geom& g)
+{
+  const int vs = g.ctuSize == 128 ? 64 : g.ctuSize, vW = (g.width + vs - 1) / vs, vx = (i % vW) * vs, vy = (i / vW) * vs, ctu = g.ctuSize;
+  if (v.x >= g.width || v.y >= g.height) return "LMCS VPDU record: CU origin outside the picture";
+  if ((v.availLeft && v.x == 0) || (v.availAbove && v.y == 0)) return "LMCS VPDU record: an available neighbour outside the picture";
+  if (v.x > vx || v.y > vy || v.x / ctu != vx / ctu || v.y / ctu != vy / ctu) return "LMCS VPDU record: CU origin not at or above-left of its VPDU in the same CTU";
+  return nullptr;
 }
 
 // ---- K3: the deblocking grid of one direction (dir 0: lfV, 1: lfH) ----

@@ -446,8 +446,6 @@ def lmcs_tables(bit_depth, min_bin, max_bin, delta_cw, chr_offset):
 def gen_lmcs(rng, bit_depth, cus, W, H, ctu, chroma_adj=True):
     """A legal random LMCS model (code words are multiples of 1 << (bd-5), so the pivot constraint of Reshape.cpp:355-363 holds) and the
     per-VPDU records: position of the CU covering each VPDU's top-left sample, neighbours available inside the picture (one slice, one tile)."""
-    from . import abi as A
-    import ctypes as C
     org = (1 << bit_depth) // 16; step = 1 << (bit_depth - 5)
     min_bin = int(rng.integers(0, 3)); max_bin = int(rng.integers(12, 16))
     while True:
@@ -456,22 +454,276 @@ def gen_lmcs(rng, bit_depth, cus, W, H, ctu, chroma_adj=True):
     delta = [int(cw[i]) - org if min_bin <= i <= max_bin else 0 for i in range(16)]
     # lmcsCW[i] + lmcsDeltaCrs must stay in [OrgCW >> 3, (OrgCW << 3) - 1] (Reshape.cpp:332-333)
     chr_off = int(rng.integers(max(-7, (org >> 3) - int(cw[min_bin:max_bin + 1].min())), 8)) if chroma_adj else 0
-    t = lmcs_tables(bit_depth, min_bin, max_bin, delta, chr_off)
+    return _lmcs_dict(bit_depth, min_bin, max_bin, delta, chr_off, chroma_adj, lmcs_vpdu_records(cus, W, H, ctu))
+
+
+def lmcs_vpdu_records(cus, W, H, ctu):
+    """The b200_lmcs_vpdu raster of a CU list: the origin of the CU covering each VPDU's top-left sample, neighbours available inside the picture
+    (one slice, one tile)."""
     vs = 64 if ctu == 128 else ctu
     vW, vH = (W + vs - 1) // vs, (H + vs - 1) // vs
-    # CU lookup on the 4x4 grid
-    owner = np.zeros(((H + 3) // 4, (W + 3) // 4), np.int32)
+    owner = np.zeros(((H + 3) // 4, (W + 3) // 4), np.int32)         # CU lookup on the 4x4 grid
     for i, (x, y, w, h) in enumerate(cus): owner[y // 4:(y + h) // 4, x // 4:(x + w) // 4] = i
     vp = np.zeros(vW * vH, LMCS_VPDU_DTYPE)
     for j in range(vH):
         for i in range(vW):
             x, y, w, h = cus[owner[j * vs // 4, i * vs // 4]]
             vp[j * vW + i] = (x, y, x > 0, y > 0)
+    return vp
+
+
+def _lmcs_dict(bit_depth, min_bin, max_bin, delta, chr_off, chroma_adj, vp):
+    from . import abi as A
+    t = lmcs_tables(bit_depth, min_bin, max_bin, delta, chr_off)
     L = A.Lmcs(); L.chromaAdj = int(chroma_adj); L.minBinIdx = min_bin; L.maxBinIdx = max_bin; L.orgCW = t["orgCW"]
     for i in range(17): L.reshapePivot[i] = t["reshapePivot"][i]; L.inputPivot[i] = t["inputPivot"][i]
     for i in range(16): L.fwdScaleCoef[i] = t["fwdScaleCoef"][i]; L.chromaAdjHelpLUT[i] = t["chromaAdjHelpLUT"][i]
     L.invLUT = t["invLUT"].ctypes.data; L.vpdus = vp.ctypes.data
     return dict(struct=L, invLUT=t["invLUT"], vpdus=vp, minBin=min_bin, maxBin=max_bin, delta=delta, chrOff=chr_off, tables=t)
+
+
+# ---- LMCS: designed models and pictures (tests/test_lmcs_*.py)
+LMCS_MODELS = ("identity", "compress", "expand_max", "fine_pivots", "narrow_bins", "single_bin", "full_bins", "crs_min", "crs_max")
+
+
+def lmcs_model_problems(bit_depth, min_bin, max_bin, delta, chr_off):
+    """The conformance checks of Reshape::constructReshaper (reference CommonLib/Reshape.cpp:331-363) and the APS syntax ranges: a list of the broken
+    rules, empty for a legal model."""
+    org = (1 << bit_depth) // 16; lo, hi, s = org >> 3, (org << 3) - 1, bit_depth - 5
+    out = []
+    if not 0 <= min_bin <= max_bin <= 15: return ["0 <= minBin <= maxBin <= 15"]
+    if not -7 <= chr_off <= 7: out.append("lmcsDeltaCrs outside -7..7")
+    cw = [delta[i] + org if min_bin <= i <= max_bin else 0 for i in range(16)]
+    for i in range(min_bin, max_bin + 1):
+        if not lo <= cw[i] <= hi: out.append(f"lmcsCW[{i}] = {cw[i]} outside {lo}..{hi}")
+        if not lo <= cw[i] + chr_off <= hi: out.append(f"lmcsCW[{i}] + lmcsDeltaCrs = {cw[i] + chr_off} outside {lo}..{hi}")
+    if sum(cw) > (1 << bit_depth) - 1: out.append(f"sum of code words {sum(cw)} above 2^bd - 1")
+    piv = [0]
+    for c in cw: piv.append(piv[-1] + c)
+    for i in range(min_bin, max_bin + 1):
+        if piv[i] % (1 << s) and piv[i] >> s == piv[i + 1] >> s: out.append(f"pivot rule at bin {i} (LmcsPivot {piv[i]} -> {piv[i + 1]})")
+    return out
+
+
+def _lmcs_design(name, bd):
+    """(minBin, maxBin, code words of bins minBin..maxBin, chroma offset) of a designed model.  A bin that starts off the 1 << (bd - 5) grid is raised
+    until it reaches the next grid line (the pivot rule, Reshape.cpp:355-363)."""
+    org = (1 << bd) // 16; step = 1 << (bd - 5); lo, hi = org >> 3, (org << 3) - 1
+    mn, mx, tg, off = {
+        "identity": (0, 14, [org] * 15, 0),                              # all 16 bins at OrgCW would sum to 2^bd, one above the limit
+        "compress": (0, 15, [org, step, org - 1, step + 1] * 4, 0),       # every code word <= OrgCW: the inverse map expands
+        "expand_max": (1, 14, [lo] * 6 + [hi] + [lo] * 7, 0),             # one bin at (OrgCW << 3) - 1, the rest at OrgCW >> 3 (raised by the pivot rule)
+        "fine_pivots": (0, 15, [step + 3, step - 1, org - 3, step + 1] * 4, 0),
+        "narrow_bins": (5, 9, [2 * org, org + step, org, 3 * step, org - step], 0),
+        "single_bin": (7, 7, [3 * org], 0),
+        "full_bins": (0, 15, [org + step, org - step] * 7 + [org, org - step], 0),
+        "crs_min": (2, 13, [lo + 7, org, org, org] * 3, -7),             # lmcsCW + lmcsDeltaCrs = OrgCW >> 3 in bins 2, 6, 10: chroma scale 16384
+        "crs_max": (4, 11, [org] * 3 + [hi - 7] + [org] * 4, 7),          # lmcsCW + lmcsDeltaCrs = (OrgCW << 3) - 1 in bin 7
+    }[name]
+    cw, p = [], 0
+    for t in tg:
+        if p % step: t = max(t, step - p % step)
+        cw.append(t); p += t
+    return mn, mx, cw, off
+
+
+def lmcs_model(name, bd, chroma_adj=True, vpdus=None):
+    """A designed LMCS model (LMCS_MODELS) at bit depth bd, in the dict gen_lmcs returns; vpdus: its b200_lmcs_vpdu raster (default: one record)."""
+    mn, mx, cw, off = _lmcs_design(name, bd)
+    org = (1 << bd) // 16
+    delta = [cw[i - mn] - org if mn <= i <= mx else 0 for i in range(16)]
+    d = _lmcs_dict(bd, mn, mx, delta, off if chroma_adj else 0, chroma_adj, np.zeros(1, LMCS_VPDU_DTYPE) if vpdus is None else vpdus)
+    d["name"] = name
+    return d
+
+
+def lmcs_fwd(m, v):
+    """The forward map (rspFwdCore, reference CommonLib/Buffer.cpp:321) of an array of samples under model dict m, before its clip to 0..2^bd - 1."""
+    t = m["tables"]; l2 = int(t["orgCW"]).bit_length() - 1
+    v = np.asarray(v, np.int64); idx = v >> l2
+    piv, inp, fwd = (np.array(t[k], np.int64) for k in ("reshapePivot", "inputPivot", "fwdScaleCoef"))
+    return piv[idx] + ((fwd[idx] * (v - inp[idx]) + (1 << 10)) >> 11)
+
+
+def lmcs_targets(m, bd):
+    """The VPDU neighbour averages the sweep aims at for model m: pivot - 1, pivot and pivot + 1 of every bin boundary minBin..maxBin + 1, 0 (below the
+    model's range) and 2^bd - 1 (above it), inside 0..2^bd - 1."""
+    piv = m["tables"]["reshapePivot"]; pmax = (1 << bd) - 1
+    t = {0, pmax}
+    for k in range(m["minBin"], m["maxBin"] + 2):
+        t |= {piv[k] - 1, piv[k], piv[k] + 1}
+    return sorted(v for v in t if 0 <= v <= pmax)
+
+
+def lmcs_vpdu_walk(v, W, H, ctu):
+    """The luma positions lmcs_vpdu_kernel sums for one VPDU record, with multiplicity (the clamps at the picture's last row / column repeat a sample):
+    dict (y, x) -> count, and the number of samples (0, n or 2n)."""
+    nn = min(64, ctu); x, y = int(v["x"]), int(v["y"])
+    pos = {}
+    for i in range(nn):
+        if v["availLeft"]: k = H - y - 1 if y + i >= H else i; pos[(y + k, x - 1)] = pos.get((y + k, x - 1), 0) + 1
+        if v["availAbove"]: k = W - x - 1 if x + i >= W else i; pos[(y - 1, x + k)] = pos.get((y - 1, x + k), 0) + 1
+    return pos, nn * (int(bool(v["availLeft"])) + int(bool(v["availAbove"])))
+
+
+def lmcs_average(luma, v, W, H, ctu, bd):
+    """The rounded neighbour average lmcs_vpdu_kernel derives for a record (1 << (bd - 1) without neighbours)."""
+    pos, n = lmcs_vpdu_walk(v, W, H, ctu)
+    if not n: return 1 << (bd - 1)
+    l2 = n.bit_length() - 1
+    return (sum(int(luma[p]) * c for p, c in pos.items()) + (n >> 1)) >> l2
+
+
+def _lmcs_place_averages(luma, vp, W, H, ctu, bd, targets):
+    """Writes the neighbourhood samples of the records in raster order so that their rounded averages take the values of `targets` (each once while
+    any is left, the ones farthest from mid-grey first, then again from the start).  Walks share samples (a VPDU's bottom-right sample is in the walks
+    of two later VPDUs), so a record takes the first target still reachable with the samples earlier records fixed."""
+    pmax = (1 << bd) - 1; fixed = set(); seen = set()
+    order = sorted(targets, key=lambda t: -abs(2 * t - pmax))
+    todo = list(order)
+    for v in vp:
+        key = (int(v["x"]), int(v["y"]))
+        pos, n = lmcs_vpdu_walk(v, W, H, ctu)
+        if not n or key in seen: continue                              # no neighbours, or a CU whose walk an earlier VPDU already set
+        seen.add(key)
+        free = sorted((p for p in pos if p not in fixed), key=lambda p: -pos[p])
+        have = sum(int(luma[p]) * c for p, c in pos.items() if p in fixed)
+        for t in (todo or order):
+            rest, left = t * n - have, sum(pos[p] for p in free)       # the rounded average is t for sums t * n - n/2 .. t * n + n/2 - 1
+            for p in free:                                              # spread the rest evenly; the last samples absorb the rounding
+                c = pos[p]; val = min(pmax, max(0, (rest + left // 2) // left))
+                luma[p] = val; rest -= val * c; left -= c
+            if lmcs_average(luma, v, W, H, ctu, bd) == t:
+                if t in todo: todo.remove(t)
+                break
+        fixed |= set(free)
+
+
+# (kind, model, bit depth, variant) of every case; names "kind_model_Nbit[_variant]"
+def _lmcs_sweep_cases():
+    out = {}
+    for bd in (8, 10, 12):
+        for m in LMCS_MODELS:
+            for st in ("stride8", "odd"): out[f"inverse_{m}_{bd}bit_{st}"] = ("inverse", m, bd, st)
+        for m in ("compress", "expand_max"): out[f"forward_{m}_{bd}bit"] = ("forward", m, bd, None)
+        out[f"vpdu_full_bins_{bd}bit_ctu32"] = ("vpdu", "full_bins", bd, "ctu32")
+        out[f"vpdu_single_bin_{bd}bit_ctu64"] = ("vpdu", "single_bin", bd, "ctu64")
+        out[f"vpdu_single_bin_{bd}bit_ctu128"] = ("vpdu", "single_bin", bd, "ctu128")
+        for adj in ("adj", "noadj"): out[f"yuv400_fine_pivots_{bd}bit_{adj}"] = ("yuv400", "fine_pivots", bd, adj)
+    out["extremes_crs_min_12bit"] = ("extremes", "crs_min", 12, None)
+    return out
+
+
+LMCS_SWEEP = _lmcs_sweep_cases()
+# CU rectangles of the VPDU cases: one CU per CTU at CTU 32 / 64 (the reference arm's structure); at CTU 128 a 128x128 CU and 64x128 CUs that
+# cover several VPDUs, and CUs whose walks reach past the picture's last row / column
+_LMCS_VPDU_GEOM = {
+    "ctu32": (256, 384, 32, None),
+    "ctu64": (200, 136, 64, None),
+    "ctu128": (232, 120, 128, [(0, 0, 128, 128), (128, 0, 64, 128), (192, 0, 32, 64), (224, 0, 32, 64), (192, 64, 64, 64)]),
+}
+
+
+def _lmcs_ramp(W, H, bd, shift=0):
+    yy, xx = np.mgrid[0:H, 0:W]
+    return ((yy * W + xx + shift) % (1 << bd)).astype(np.int16)
+
+
+def _lmcs_case(name):
+    from . import abi as A
+    import ctypes as C, zlib
+    kind, model, bd, var = LMCS_SWEEP[name]
+    rng = np.random.default_rng(zlib.crc32(name.encode()))
+    pmax, mid = (1 << bd) - 1, 1 << (bd - 1)
+    chroma = kind != "yuv400"
+    cus, pus, tus, coefs, tags = None, np.zeros(0, PU_DTYPE), np.zeros(0, A.TU_DTYPE), np.zeros(1, np.int16), []
+    if kind == "inverse":                                               # a ramp of every value as `given` luma: the output is invLUT[v]
+        W, H, ctu = 64, 64, 64
+        strides = (64, 32, 32) if var == "stride8" else (67, 35, 35)
+        given = [np.full((H, strides[0]), -7, np.int16)] + [np.full((H // 2, strides[c]), -7, np.int16) for c in (1, 2)]
+        given[0][:, :W] = _lmcs_ramp(W, H, bd); given[1][:, :W // 2] = mid; given[2][:, :W // 2] = mid // 2
+    elif kind == "vpdu":
+        W, H, ctu, cus = _LMCS_VPDU_GEOM[var]
+        strides = None
+    elif kind == "extremes":
+        W, H, ctu, strides = 128, 128, 32, None
+    else:
+        W, H, ctu, strides = 64, 64, 64, None
+    if cus is None: cus = [(x, y, min(ctu, W - x), min(ctu, H - y)) for y in range(0, H, ctu) for x in range(0, W, ctu)]
+    vp = lmcs_vpdu_records(cus, W, H, ctu)
+    m = lmcs_model(model, bd, chroma_adj=var != "noadj", vpdus=vp)
+    g = A.make_geom(W, H, bd, chroma_format=1 if chroma else 0, ctu=ctu, strides=strides)
+    dpb = [noise_planes(rng, W, H, bd, strides=strides) for _ in range(4)]
+    if kind in ("forward", "yuv400"):
+        # the ramp in slot 0, copied by zero-MV uni PUs of several sizes and by one bi PU whose two references are slot 0 (integer MVs: the bi average of
+        # two equal predictions is exact); no DMVR / BDOF, no residual on the forward cases
+        dpb[0][0][:] = _lmcs_ramp(W, H, bd, shift=17)
+        rects = [(0, 0, 32, 32, "bi")] + [(32 + 16 * (i % 2), 16 * (i // 2), 16, 16, "uni") for i in range(4)] + \
+                [(0, 32 + 8 * j, 32, 8, "uni") for j in range(2)] + [(8 * i, 48, 8, 16, "uni") for i in range(4)] + \
+                [(32 + 8 * (i % 4), 32 + 8 * (i // 4), 8, 8, "uni") for i in range(16)]
+        pus = np.zeros(len(rects), PU_DTYPE)
+        for r, (x, y, w, h, kd) in zip(pus, rects):
+            r["x"], r["y"], r["w"], r["h"], r["bcwW1"] = x, y, w, h, 4
+            if kd == "bi": r["refSlot"] = (0, 0); r["interDir"] = 3
+            else: r["refSlot"] = (0, -1); r["interDir"] = 1
+            tags.append(f"{kd} PU {w}x{h} at ({x}, {y})")
+        given = None
+        if kind == "yuv400":                                            # luma TUs on top: residual added in the mapped domain
+            b = _K1Case(W, bd, rng)
+            ts = dict(flags=A.TU_TS, qp=4 - 6 * (bd - 8))
+            for k, (x, y) in enumerate([(0, 0), (8, 8), (40, 40), (56, 0)]):
+                b.add(f"luma TS 8x8 at ({x}, {y})", 0, 8, 8, rng.integers(-pmax // 4, pmax // 4 + 1, (8, 8)), at=(x, y), **ts)
+            tus, coefs = np.array(b.recs, A.TU_DTYPE), np.concatenate(b.levels); tags += b.tags
+    else:
+        if kind != "inverse":                                           # designed luma neighbourhoods + chroma TUs that show each VPDU's scale
+            luma = np.full((H, W), mid, np.int16)
+            vs = 64 if ctu == 128 else ctu
+            if kind == "extremes":                                      # every average inside a bin whose chroma scale is 16384
+                piv = m["tables"]["reshapePivot"]; bins = [i for i in range(16) if m["tables"]["chromaAdjHelpLUT"][i] == 16384]
+                targets = [piv[b] + k for b in bins for k in range(3)]
+            else:
+                targets = lmcs_targets(m, bd)
+            _lmcs_place_averages(luma, vp, W, H, ctu, bd, targets)
+            given = [luma, np.full((H // 2, W // 2), mid, np.int16), np.full((H // 2, W // 2), mid, np.int16)]
+            b = _K1Case(W, bd, rng)
+            ts = dict(flags=A.TU_TS, qp=4 - 6 * (bd - 8))
+            vW = (W + vs - 1) // vs
+            for k, v in enumerate(vp):
+                cx, cy = (k % vW) * vs // 2, (k // vW) * vs // 2
+                cw, ch = min(vs // 2, W // 2 - cx), min(vs // 2, H // 2 - cy)
+                R = [1 << bd, -(1 << bd), 4095, -4096][k % 4] if kind == "extremes" else (37 + 11 * k) % (mid // 2) + 5
+                big = 8 if min(cw, ch) >= 8 else 4
+                b.add(f"VPDU {k} Cb DC {big}x{big}", 1, big, big, np.full((big, big), R), at=(cx, cy), **ts)
+                b.add(f"VPDU {k} Cr DC {big}x{big}", 2, big, big, np.full((big, big), -R), at=(cx, cy), **ts)
+                if cw >= big + 4 and ch >= 4:
+                    ict = (1, -1, 2, -2, 3, -3)[k % 6]
+                    b.add(f"VPDU {k} joint CbCr 4x4 ict {ict}", 1 + (abs(ict) == 3), 4, 4, np.full((4, 4), R), at=(cx + big, cy), ict=ict, **ts)
+                if ch >= big + 2:
+                    b.add(f"VPDU {k} Cb 2x2 (4 samples, unscaled)", 1, 2, 2, np.full((2, 2), R), at=(cx, cy + big), **ts)
+                    b.add(f"VPDU {k} Cr 2x2 (4 samples, unscaled)", 2, 2, 2, np.full((2, 2), -R), at=(cx, cy + big), **ts)
+            tus, coefs = np.array(b.recs, A.TU_DTYPE), np.concatenate(b.levels); tags += b.tags
+    if not chroma:
+        g.stride[1] = g.stride[2] = 0
+        dpb = [[p[0], np.zeros((H // 2, W // 2), np.int16), np.zeros((H // 2, W // 2), np.int16)] for p in dpb]
+    p = A.Picture(); p.dstSlot = 4; p.flags = A.PIC_LMCS; p.lmcs = C.addressof(m["struct"])
+    d = dict(pus=pus, ndmvr=0, tus=tus, coefs=coefs, lmcs=m)
+    p.pus = pus.ctypes.data; p.numPus = len(pus); p.numDmvr = 1
+    p.tus = tus.ctypes.data; p.numTus = len(tus); p.coefs = coefs.ctypes.data; p.numCoefs = len(coefs)
+    if given is not None:
+        d["given"] = given
+        for c in range(3 if chroma else 1): p.given[c] = given[c].ctypes.data
+    d["struct"] = p
+    return dict(name=name, kind=kind, model=model, bd=bd, variant=var, g=g, W=W, H=H, ctu=ctu, chroma=chroma, strides=strides, cus=cus, dpb=dpb,
+                pic=d, tags=tags)
+
+
+def lmcs_sweep(name):
+    """One case of the designed LMCS sweep (LMCS_SWEEP): geometry (g, W, H, bd, ctu, chroma, strides), CU rectangles, DPB slots (4 x [Y, Cb, Cr]), the
+    picture dict (pic: pus, tus, coefs, given, lmcs = the model dict, struct = the b200_picture, destination slot 4, filters off) and per-record tags.
+    inverse: a ramp of every value as `given` luma, no PUs / TUs; forward: the ramp copied by zero-MV uni and bi PUs; vpdu: designed neighbour averages
+    and one DC chroma TU per VPDU (with 4-sample and joint-CbCr TUs); extremes: residuals of +-2^bd scaled by 16384 at 12 bit; yuv400: 4:0:0 with
+    PUs and luma TUs, chroma scaling on / off."""
+    return _lmcs_case(name)
 
 
 def gen_picture(rng, W, H, bit_depth=10, ctu=128, dst_slot=0, cu_kw=None, pu_kw=None, tu_kw=None, sao_p=0.4, alf_kw=None,
