@@ -18,4 +18,3 @@ for name, case in (("B", wl.B[0]), ("I", wl.I)):
     for _ in range(5): vvdec_b200.check(lib.b200_pic_run(ctx, h))
     vvdec_b200.check(lib.b200_ctx_mark(ctx, 1)); t = C.c_float(); vvdec_b200.check(lib.b200_ctx_elapsed_ms(ctx, C.byref(t)))
     print(name, "picture ms", t.value / 5, "intra blocks", len(pic.get("intraTus", [])), flush=True)
-    if hasattr(lib, "b200_k6_prof_dump"): lib.b200_k6_prof_dump(1)
