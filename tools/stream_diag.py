@@ -1,6 +1,6 @@
 """Diagnosis of a stream that decodes differently through the swapped decoder (test infrastructure): for a seed of tools/stream_fuzz.py (optionally with
 overridden configuration entries, e.g. deblocking_disabled=True sao=False to take the in-loop filters out), prints for the first picture that differs a map of the
-differing 8x8 blocks per plane and the flattened PU / TU / intra records that cover the first differing sample.
+differing 8x8 blocks per plane and the flattened PU / TU / intra records that cover the first differing sample (stream_util.describe_difference).
     python tools/stream_diag.py SEED [key=value ...]"""
 import sys, numpy as np
 import os
@@ -14,43 +14,24 @@ kw, pics, st = sf.random_case(seed)
 for a in sys.argv[2:]:
     k, v = a.split("="); kw[k] = eval(v)
 aus, drawn, nb = vs.build_stream(vs.Config(**kw), pics, seed=seed)
-keep = {}
+keep = []
 stock = vs.decode(vs.REF_SO, aus); sw, log = su.decode_swapped_cpu(aus, oracle, keep=keep)
-order = sorted(range(len(pics)), key=lambda i: pics[i].poc)
+frame = vs.output_order(pics)                                       # decoding index -> output index
 np.set_printoptions(linewidth=250)
-for oi, (a, b) in enumerate(zip(sw, stock)):
+for i, rec in sorted(enumerate(keep), key=lambda e: frame[e[0]]):
+    a, b = sw[frame[i]], stock[frame[i]]
     if all((x == y).all() for x, y in zip(a, b)): continue
-    poc = pics[order[oi]].poc; pic = keep[poc]
-    print("poc", poc, "slice types", pics[order[oi]].slice_type, pics[order[oi]].slice_types)
+    pic = rec["pic"]
+    print("poc", rec["poc"], "slice types", pics[i].slice_type, pics[i].slice_types)
     for c in range(3):
-        d = (a[c] != b[c]); 
+        d = (a[c] != b[c])
         if not d.any(): continue
         B = 8 if c == 0 else 4
         H, W = d.shape; g = d[:H // B * B, :W // B * B].reshape(H // B, B, W // B, B).any(axis=(1, 3))
-        print("plane", c, "blocks (8x8 luma units) with diffs:"); 
+        print("plane", c, "blocks (8x8 luma units) with diffs:")
         for r in range(g.shape[0]):
             if g[r].any(): print("%3d " % (r * 8), "".join("#" if v else "." for v in g[r]))
-    pus = pic["pus"]; tus = pic["tus"]; it = pic.get("intraTus")
-    d = np.argwhere(a[0] != b[0])
-    if not len(d): d = np.argwhere(a[1] != b[1]) * 2
-    y, x = d[np.lexsort((d[:, 1], d[:, 0]))][0]
-    print("first diff at", x, y)
-    print("PUs:", pus[(pus["x"] <= x) & (x < pus["x"] + pus["w"].astype(int)) & (pus["y"] <= y) & (y < pus["y"] + pus["h"].astype(int))])
-    tw = 1 << tus["log2w"].astype(int); th = 1 << tus["log2h"].astype(int); sc = np.where(tus["comp"] == 0, 1, 2)
-    m = (tus["x"] * sc <= x) & (x < (tus["x"] + tw) * sc) & (tus["y"] * sc <= y) & (y < (tus["y"] + th) * sc)
-    print("TUs:", tus.dtype.names); print(tus[m])
-    if it is not None:
-        iw = 1 << it["log2w"].astype(int); ih = 1 << it["log2h"].astype(int); sc = np.where(it["comp"] == 0, 1, 2)
-        m = (it["x"] * sc <= x) & (x < (it["x"] + iw) * sc) & (it["y"] * sc <= y) & (y < (it["y"] + ih) * sc)
-        print("intra:", it.dtype.names); print(it[m])
-    pass
-    for (qx, qy) in ((96, 124), (64, 121)):
-        print("--- records at", qx, qy)
-        print(pus[(pus["x"] <= qx) & (qx < pus["x"] + pus["w"].astype(int)) & (pus["y"] <= qy) & (qy < pus["y"] + pus["h"].astype(int))])
-        tw = 1 << tus["log2w"].astype(int); th = 1 << tus["log2h"].astype(int); sc = np.where(tus["comp"] == 0, 1, 2)
-        print(tus[(tus["x"] * sc <= qx) & (qx < (tus["x"] + tw) * sc) & (tus["y"] * sc <= qy) & (qy < (tus["y"] + th) * sc)])
-        if it is not None:
-            iw = 1 << it["log2w"].astype(int); ih = 1 << it["log2h"].astype(int); sc = np.where(it["comp"] == 0, 1, 2)
-            print(it[(it["x"] * sc <= qx) & (qx < (it["x"] + iw) * sc) & (it["y"] * sc <= qy) & (qy < (it["y"] + ih) * sc)])
+    print(su.describe_difference(pic, a, b, 3 if rec["geom"].chromaFormat else 1))
     print("alf ctus", pic["alf"]["ctus"] if "alf" in pic else None)
     print("sao", pic.get("sao"))
+    break
