@@ -412,7 +412,8 @@ enum { B200_PIC_DEBLOCK = 1, B200_PIC_SAO = 2, B200_PIC_ALF = 4, B200_PIC_LMCS =
  * invalid geometry (b200_geom). */
 B200_API int  b200_ctx_create(b200_ctx** ctx, const b200_geom* g, int numSlots, int numArenas, int device);
 B200_API void b200_ctx_destroy(b200_ctx* ctx);
-/* Host planes -> DPB slot (e.g. an IRAP picture reconstructed elsewhere, or test content). Synchronous. */
+/* Host planes -> DPB slot (e.g. an IRAP picture reconstructed elsewhere, or test content). Synchronous; waits for pending asynchronous outputs of the
+ * slot's buffer before it overwrites it. */
 B200_API int  b200_ctx_load_slot(b200_ctx* ctx, int slot, const int16_t* const planes[3]);
 /* decompressPicture() = b200_pic_upload + b200_pic_run.  Returns the arena handle (>= 0) or a negative error.
  *
@@ -422,9 +423,10 @@ B200_API int  b200_ctx_load_slot(b200_ctx* ctx, int slot, const int16_t* const p
  *   B200_ERR_PARAM for the geometry, ALF table counts and virtual boundaries b200_sao_picture / b200_alf_picture refuse.
  * b200_pic_run: enqueues the picture's kernel chain.  It sizes the grids from the list lengths the upload produced, so it waits (host)
  *   until that upload has finished; a caller that uploads picture n+1 before it runs picture n (a parser running ahead of
- *   reconstruction) never waits.  An invalid record (reference slot outside the DPB, impossible block size, BDOF/DMVR on a block that
+ *   reconstruction) never waits.  Once it returns the picture's upload is complete: the caller may overwrite or free the host arrays.  An invalid record (reference slot outside the DPB, impossible block size, BDOF/DMVR on a block that
  *   cannot have it, DMVR at more than 10 bit) makes it return B200_ERR_PARAM without running anything.
- * A handle may be run several times (device-resident benchmarking). */
+ * A handle may be run several times (device-resident benchmarking); it keeps its work lists until its arena is uploaded again (numArenas uploads
+ * later), and that upload waits on the device for the kernels of the handle's last run. */
 B200_API int  b200_decompress_picture(b200_ctx* ctx, const b200_picture* pic);
 B200_API int  b200_pic_upload(b200_ctx* ctx, const b200_picture* pic);            /* -> arena handle */
 B200_API int  b200_pic_run(b200_ctx* ctx, int arena);
@@ -440,7 +442,9 @@ B200_API int  b200_get_frame(b200_ctx* ctx, int slot, int16_t* const planes[3]);
 B200_API int  b200_ctx_load_slot_strided(b200_ctx* ctx, int slot, const int16_t* const planes[3], const ptrdiff_t strides[3]);
 B200_API int  b200_get_frame_strided(b200_ctx* ctx, int slot, int16_t* const planes[3], const ptrdiff_t strides[3]);
 /* Asynchronous output: the D2H copy runs on a second stream after the picture is final and overlaps the next pictures' kernels;
- * the context makes later pictures wait before they overwrite a buffer that is still being read.  Returns a ticket (>= 0);
+ * the context makes later pictures (and b200_ctx_load_slot*) wait before they overwrite a buffer that is still being read — by every pending
+ * reader, whichever output call and stream it came from (two readers on different streams: the later one's stream first waits for the earlier
+ * one).  Returns a ticket (>= 0);
  * b200_frame_wait(ticket) blocks until those planes are complete in host memory (pinned memory recommended). */
 B200_API int  b200_get_frame_async(b200_ctx* ctx, int slot, int16_t* const planes[3]);
 B200_API int  b200_frame_wait(b200_ctx* ctx, int ticket);
@@ -471,7 +475,8 @@ typedef struct b200_film_grain {
   uint8_t         scaleShift;    /* FilmGrainImpl::scale_shift after set_depth / set_scale_shift; scaleShift + bitDepth - 8 in 8..13       */
   uint8_t         compPresent[3];/* fgs.comp_model_present_flag                                                                            */
 } b200_film_grain;
-/* Like b200_get_frame_fmt_async, with grain added before the format conversion.  The arrays are copied before the call returns. */
+/* Like b200_get_frame_fmt_async, with grain added before the format conversion.  The arrays are copied (into pinned memory of the context) before
+ * the call returns: the caller may overwrite them at once. */
 B200_API int  b200_get_frame_grain_async(b200_ctx* ctx, int slot, int fmt, void* const planes[3], const b200_film_grain* fg);
 /* Decoded-picture hash computed on the device (SURVEY 8f-3): what calcCRC / calcChecksum (CommonLib/PicYuvMD5.cpp:138,:179) produce for
  * the decoded picture hash SEI check (calcAndPrintHashStatus :261), so a verify-only run reads back 6 / 12 bytes instead of the frame.

@@ -1,5 +1,5 @@
 """Test helpers: load the oracle (C restatement) and, when built, the reference shim."""
-import contextlib, os, subprocess, ctypes as C
+import contextlib, functools, os, subprocess, ctypes as C
 import numpy as np
 from vvdec_b200 import abi, synth
 
@@ -512,6 +512,68 @@ def intra_case(W, H, ctu, seed, min_size=8, bd=10, chroma=True, strides=None, p_
     resi = [rng.integers(-40, 41, size=p.shape).astype(np.int16) for p in planes]
     if not chroma: planes, resi = planes + [None, None], resi + [None, None]
     return g, planes, resi, recs
+
+
+# ---- pictures in flight (tests/test_pipeline_*.py): short schedules of synthetic pictures with a DPB slot plan
+# Kinds: I an intra picture (dense list: the CTU-resident K6 kernel), B a B picture with sparse intra blocks and CIIP blocks that carry a residual (the
+# one-CTA-per-block kernel and the CIIP clear), L the same with LMCS and chroma scaling (K6 in two passes), P inter only (DMVR on many PUs), p a small
+# inter picture (large CUs, few records).  Filters: D deblocking, S SAO, A ALF ('-': off).  Every picture references DPB slots 0..3.
+PIPELINE_KINDS = {
+    "I": dict(intra_frac=1.0),
+    "B": dict(intra_frac=0.05, p_ciip=0.1, cu_kw=dict(min_size=16)),
+    "L": dict(intra_frac=0.05, p_ciip=0.1, cu_kw=dict(min_size=16), lmcs=True, lmcs_chroma=True),
+    "P": dict(pu_kw=dict(p_dmvr=0.6)),
+    "p": dict(cu_kw=dict(min_dim=32, min_area=1024)),
+}
+PIPELINE_SLOTS = 6
+PIPELINE_SCHEDULES = {   # name -> (W, H, seed, [(kind, dstSlot, filters)])
+    "416x240": (416, 240, 1, [("I", 4, "DSA"), ("B", 5, "D-A"), ("B", 5, "DS-"), ("L", 0, "DSA"), ("P", 1, "---"), ("B", 2, "D--"), ("P", 4, "DSA"), ("L", 3, "-SA")]),
+    "832x480": (832, 480, 2, [("P", 4, "DSA"), ("I", 5, "DSA"), ("B", 0, "D-A"), ("L", 0, "---"), ("P", 1, "DS-"), ("B", 4, "DSA")]),
+    "1920x1080": (1920, 1080, 3, [("I", 4, "DSA"), ("B", 5, "DSA"), ("P", 0, "D--")]),
+    # small inter pictures first, then larger lists into the same arenas; the first intra picture arrives while the inter pictures are in flight
+    "grow_416x240": (416, 240, 4, [("p", 4, "---"), ("p", 5, "---"), ("B", 4, "DSA"), ("L", 5, "DSA"), ("I", 0, "DSA")]),
+}
+
+
+@functools.lru_cache(maxsize=None)
+def pipeline_schedule(name):
+    """The pictures of PIPELINE_SCHEDULES[name]: a dict with g, W, H, the initial DPB (PIPELINE_SLOTS noise pictures), kinds, dsts and pics
+    (synth.gen_picture dicts, struct.dstSlot set)."""
+    W, H, seed, steps = PIPELINE_SCHEDULES[name]
+    rng = np.random.default_rng(seed)
+    bd = 10
+    dpb = [synth.noise_planes(rng, W, H, bd) for _ in range(PIPELINE_SLOTS)]
+    pics = [synth.gen_picture(rng, W, H, bd, dst_slot=dst, deblock="D" in f, sao="S" in f, alf="A" in f, **PIPELINE_KINDS[k]) for k, dst, f in steps]
+    return dict(name=name, g=abi.make_geom(W, H, bd), W=W, H=H, bd=bd, dpb=dpb, kinds=[k for k, _, _ in steps], dsts=[d for _, d, _ in steps], pics=pics)
+
+
+def pipeline_refs(pic):
+    """DPB slots the picture's PUs read."""
+    r = pic["pus"]["refSlot"].ravel()
+    return set(int(v) for v in r[r >= 0])
+
+
+def arena_bytes(g, pic):
+    """Size of the arena b200_pic_upload lays out for the picture (picture.cu: every array at a 256-byte boundary, 16 bytes of slack)."""
+    a = lambda n: (n + 16 + 255) & ~255
+    st = pic["struct"]
+    n4 = ((g.width + 3) >> 2) * ((g.height + 3) >> 2)
+    nctu = ((g.width + g.ctuSize - 1) // g.ctuSize) * ((g.height + g.ctuSize - 1) // g.ctuSize)
+    db, sao, alf, lm = st.flags & abi.PIC_DEBLOCK, st.flags & abi.PIC_SAO, st.flags & abi.PIC_ALF, st.flags & abi.PIC_LMCS
+    tab = 0
+    if alf:
+        t = pic["alf"]; tab = 2 * (2 * len(t["lumaCoeff"]) * 1300 + 2 * len(t["chromaCoeff"]) * 7 + len(t["cc"][0]) * 7 + len(t["cc"][1]) * 7)
+    vs = 64 if g.ctuSize == 128 else g.ctuSize
+    nv = ((g.width + vs - 1) // vs) * ((g.height + vs - 1) // vs)
+    ni = int(st.numIntraTus)
+    sizes = [st.numPus * 64, n4 * 4, 2 * 128 * 4, st.numTus * 4, st.numTus * 32, st.numCoefs * 2, st.numScaling * 4, n4 * 6 if db else 0, n4 * 6 if db else 0, nctu,
+             nctu * 24 if sao else 0, nctu * 8 if alf else 0, tab, st.numDmvr * 8, st.numWp * 24, C.sizeof(abi.Lmcs) if lm else 0, (2 << g.bitDepth) if lm else 0,
+             nv * 6 if lm else 0, nv * 4 if lm else 0, 0, ni * 16, (ni + 2) * 4 if ni else 0, (ni + 8 + 3 * nctu) * 4 if ni else 0]
+    if ni:
+        for k in range(3 if g.chromaFormat else 1):
+            pw, ph, unit = (g.width, g.height, 4) if k == 0 else (g.width >> 1, g.height >> 1, 2)
+            sizes.append(((pw + unit - 1) // unit) * ((ph + unit - 1) // unit) * 4)
+    return sum(a(s) for s in sizes)
 
 
 # ---- K2: one comparison for every MC test (tests/test_k2_*.py)

@@ -47,7 +47,8 @@ struct b200_ctx {
   cudaStream_t stream = nullptr, copyStream = nullptr, upStream = nullptr;   // kernels / frame output D2H / work-list H2D
   StreamSet ss;
   cudaEvent_t ev[2] = {nullptr, nullptr};
-  std::vector<cudaEvent_t> readDone; std::vector<char> readPending;   // per picture buffer: an async D2H is (maybe) still reading it
+  std::vector<cudaEvent_t> readDone; std::vector<char> readPending;   // per picture buffer: an async output (maybe) still reads it (mark_read)
+  std::vector<cudaStream_t> readStream;                              // the stream readDone was last recorded on
   cudaEvent_t ticketEv[16]; cudaEvent_t finalEv = nullptr; int nextTicket = 0;
   DevBuf outStage[2]; int nextStage = 0;   // converted output frames (pyuv / 8 bit) waiting for their D2H copy
   size_t planeBytes[3] = {0, 0, 0}, picBytes = 0;
@@ -58,6 +59,7 @@ struct b200_ctx {
   int nextArena = 0;
   long long launches = 0;
   DevBuf grainStage[2], grainTab;    // b200_get_frame_grain_async: grained copy of the frame, device copies of the tables + block seeds
+  struct HostStage { void* p = nullptr; size_t cap = 0; cudaEvent_t copied = nullptr; bool pending = false; } grainHost[2];   // pinned copies of the caller's tables
   DevBuf resiBuf;                    // residual planes of intra CUs (K1 -> K6), allocated with the first picture that carries intra blocks
   DevBuf hashBuf;                    // b200_frame_hash_async: accumulators + digest per ticket
 
@@ -74,6 +76,23 @@ extern "C" {
 static int copy2d_host(void* dst, size_t dpitch, const void* src, size_t spitch, size_t wBytes, size_t h, cudaMemcpyKind kind, cudaStream_t s);
 // a contiguous copy between caller memory and the device (see copy2d_host: the caller's array may start in a page registered for another array)
 static inline int copy_host(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t s) { return copy2d_host(dst, bytes, src, bytes, bytes, 1, kind, s); }
+
+// Ordering of the picture buffers and their asynchronous readers (the output calls): readDone[buf] is where the last reader of buffer `buf` is done.  A
+// reader on stream s records it after its own work; when a reader on another stream is still pending, s first waits for that one, so the one event covers
+// both (s's later work then waits for it too).  b200_pic_run (for its two work buffers) and b200_ctx_load_slot* wait for readDone before they write a buffer.
+static int mark_read(b200_ctx* c, int buf, cudaStream_t s)
+{
+  if (c->readPending[buf] && c->readStream[buf] != s) B200_CUDA(cudaStreamWaitEvent(s, c->readDone[buf], 0));
+  B200_CUDA(cudaEventRecord(c->readDone[buf], s));
+  c->readPending[buf] = 1; c->readStream[buf] = s;
+  return 0;
+}
+
+static int wait_readers(b200_ctx* c, int buf)
+{
+  if (c->readPending[buf]) { B200_CUDA(cudaStreamWaitEvent(c->stream, c->readDone[buf], 0)); c->readPending[buf] = 0; }
+  return 0;
+}
 
 B200_API int b200_ctx_create(b200_ctx** out, const b200_geom* g, int numSlots, int numArenas, int device)
 {
@@ -97,8 +116,9 @@ B200_API int b200_ctx_create(b200_ctx** out, const b200_geom* g, int numSlots, i
   for (int k = 0; k < 3; k++) c->planeBytes[k] = (k == 0 || g->chromaFormat) ? align256((size_t)g->stride[k] * (k ? g->height >> 1 : g->height) * 2) : 0;
   c->picBytes = c->planeBytes[0] + c->planeBytes[1] + c->planeBytes[2];
   c->bufs.resize(numSlots + 2); c->slotBuf.resize(numSlots);
-  c->readDone.resize(numSlots + 2); c->readPending.assign(numSlots + 2, 0);
+  c->readDone.resize(numSlots + 2); c->readPending.assign(numSlots + 2, 0); c->readStream.assign(numSlots + 2, nullptr);
   for (auto& e : c->readDone) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  for (auto& h : c->grainHost) B200_CUDA(cudaEventCreateWithFlags(&h.copied, cudaEventDisableTiming));
   for (int i = 0; i < numSlots + 2; i++) { B200_CUDA(cudaMalloc(&c->bufs[i], c->picBytes)); B200_CUDA(cudaMemset(c->bufs[i], 0, c->picBytes)); }
   for (int s = 0; s < numSlots; s++) c->slotBuf[s] = s;
   c->work[0] = numSlots; c->work[1] = numSlots + 1;
@@ -117,6 +137,7 @@ B200_API void b200_ctx_destroy(b200_ctx* c)
   for (auto p : c->bufs) cudaFree(p);
   for (auto e : c->readDone) cudaEventDestroy(e);
   for (auto e : c->ticketEv) cudaEventDestroy(e);
+  for (auto& h : c->grainHost) { cudaEventDestroy(h.copied); if (h.p) cudaFreeHost(h.p); }
   cudaEventDestroy(c->finalEv); cudaStreamDestroy(c->copyStream);
   for (int k = 0; k < c->ss.nAux; k++) { cudaStreamSynchronize(c->ss.aux[k]); cudaStreamDestroy(c->ss.aux[k]); cudaEventDestroy(c->ss.joinEv[k]); }
   cudaEventDestroy(c->ss.forkEv);
@@ -128,6 +149,7 @@ B200_API void b200_ctx_destroy(b200_ctx* c)
 B200_API int b200_ctx_load_slot(b200_ctx* c, int slot, const int16_t* const planes[3])
 {
   B200_CHECK(c && planes && slot >= 0 && slot < c->numSlots, "b200_ctx_load_slot: bad argument");
+  if (int rc = wait_readers(c, c->slotBuf[slot])) return rc;
   DevPlanes d = c->planes(c->slotBuf[slot]);
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++)
     if (int rc = copy_host(d.p[k], planes[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyHostToDevice, c->stream)) return rc;
@@ -285,7 +307,7 @@ B200_API int b200_pic_run(b200_ctx* c, int ai)
   B200_CUDA(cudaStreamWaitEvent(s, A.uploaded, 0));
   const b200_geom& g = c->g;
   int cur = c->work[0], other = c->work[1];
-  for (int b : {cur, other}) if (c->readPending[b]) { B200_CUDA(cudaStreamWaitEvent(s, c->readDone[b], 0)); c->readPending[b] = 0; }   // async output copies still reading these buffers
+  for (int b : {cur, other}) if (int rc = wait_readers(c, b)) return rc;   // async outputs still reading these buffers
   DevPlanes P = c->planes(cur);
   // 0. pre-reconstructed (intra stand-in) samples
   if (A.given[0]) {
@@ -442,6 +464,7 @@ static int copy2d_host(void* dst, size_t dpitch, const void* src, size_t spitch,
 B200_API int b200_ctx_load_slot_strided(b200_ctx* c, int slot, const int16_t* const planes[3], const ptrdiff_t strides[3])
 {
   B200_CHECK(c && planes && strides && slot >= 0 && slot < c->numSlots, "b200_ctx_load_slot_strided: bad argument");
+  if (int rc = wait_readers(c, c->slotBuf[slot])) return rc;
   DevPlanes d = c->planes(c->slotBuf[slot]);
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++) {
     const size_t w = k ? c->g.width >> 1 : c->g.width, h = k ? c->g.height >> 1 : c->g.height;
@@ -474,7 +497,7 @@ B200_API int b200_get_frame_async(b200_ctx* c, int slot, int16_t* const planes[3
   B200_CUDA(cudaStreamWaitEvent(c->copyStream, c->finalEv, 0));
   for (int k = 0; k < (c->g.chromaFormat ? 3 : 1); k++)
     if (int rc = copy_host(planes[k], d.p[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyDeviceToHost, c->copyStream)) return rc;
-  B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;
+  if (int rc = mark_read(c, buf, c->copyStream)) return rc;
   const int t = c->nextTicket; c->nextTicket = (c->nextTicket + 1) & 15;
   B200_CUDA(cudaEventRecord(c->ticketEv[t], c->copyStream));
   return t;
@@ -494,7 +517,7 @@ B200_API int b200_get_frame_device_async(b200_ctx* c, int slot, int16_t* const p
     B200_CHECK(planesDev[k], "b200_get_frame_device_async: plane %d", k);
     B200_CUDA(cudaMemcpyAsync(planesDev[k], d.p[k], (size_t)c->g.stride[k] * (k ? c->g.height >> 1 : c->g.height) * 2, cudaMemcpyDeviceToDevice, st));
   }
-  B200_CUDA(cudaEventRecord(c->readDone[buf], st)); c->readPending[buf] = 1;
+  if (int rc = mark_read(c, buf, st)) return rc;
   return 0;
 }
 
@@ -527,7 +550,7 @@ B200_API int b200_get_frame_fmt_async(b200_ctx* c, int slot, int fmt, void* cons
   uint8_t* dst[3]; for (int k = 0; k < 3; k++) dst[k] = c->outStage[st].as<uint8_t>() + off[k];
   if (int rc = launch_pack(d, c->g, fmt, dst, c->copyStream)) return rc;                      // on the copy stream: the kernel stream runs on
   c->launches += nPl;
-  B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;       // the picture buffer is free once it is packed
+  if (int rc = mark_read(c, buf, c->copyStream)) return rc;                                   // the picture buffer is free once it is packed
   for (int k = 0; k < nPl; k++) if (int rc = copy_host(planes[k], dst[k], bytes[k], cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   const int t = c->nextTicket; c->nextTicket = (c->nextTicket + 1) & 15;
   B200_CUDA(cudaEventRecord(c->ticketEv[t], c->copyStream));
@@ -555,10 +578,19 @@ B200_API int b200_get_frame_grain_async(b200_ctx* c, int slot, int fmt, void* co
   if (int rc = c->grainTab.reserve(tabBytes)) return rc;
   if (int rc = c->grainStage[st].reserve(c->picBytes)) return rc;
   uint8_t* tb = c->grainTab.as<uint8_t>();
-  if (int rc = copy_host(tb, fg->pattern, oS, cudaMemcpyHostToDevice, c->copyStream)) return rc;
-  if (int rc = copy_host(tb + oS, fg->sLUT, 768, cudaMemcpyHostToDevice, c->copyStream)) return rc;
-  if (int rc = copy_host(tb + oP, fg->pLUT, 768, cudaMemcpyHostToDevice, c->copyStream)) return rc;
-  if (int rc = copy_host(tb + oL, fg->lineSeeds, (size_t)nby * 4, cudaMemcpyHostToDevice, c->copyStream)) return rc;
+  // The caller may reuse its arrays once this call returns, while the H2D copy may still wait behind earlier work of the copy stream: the tables go through
+  // pinned memory of the context first.  Stage st is refilled once the copy of the call before last that used it has run.
+  auto& hs = c->grainHost[st];
+  if (hs.pending) { B200_CUDA(cudaEventSynchronize(hs.copied)); hs.pending = false; }
+  if (oB > hs.cap) {
+    if (hs.p) cudaFreeHost(hs.p);
+    hs.p = nullptr; hs.cap = 0;
+    B200_CUDA(cudaHostAlloc(&hs.p, oB, cudaHostAllocDefault)); hs.cap = oB;
+  }
+  uint8_t* hb = static_cast<uint8_t*>(hs.p);
+  memcpy(hb, fg->pattern, oS); memcpy(hb + oS, fg->sLUT, 768); memcpy(hb + oP, fg->pLUT, 768); memcpy(hb + oL, fg->lineSeeds, (size_t)nby * 4);
+  B200_CUDA(cudaMemcpyAsync(tb, hb, oB, cudaMemcpyHostToDevice, c->copyStream));
+  B200_CUDA(cudaEventRecord(hs.copied, c->copyStream)); hs.pending = true;
   const int buf = c->slotBuf[slot];
   DevPlanes src = c->planes(buf), gr = src;
   { uint8_t* b = c->grainStage[st].as<uint8_t>(); gr.p[0] = reinterpret_cast<int16_t*>(b); gr.p[1] = reinterpret_cast<int16_t*>(b + c->planeBytes[0]); gr.p[2] = reinterpret_cast<int16_t*>(b + c->planeBytes[0] + c->planeBytes[1]); }
@@ -567,7 +599,7 @@ B200_API int b200_get_frame_grain_async(b200_ctx* c, int slot, int fmt, void* co
   if (int rc = launch_film_grain(src, gr, g, reinterpret_cast<const int8_t*>(tb), tb + oS, tb + oP, reinterpret_cast<const uint32_t*>(tb + oL),
                                  reinterpret_cast<uint32_t*>(tb + oB), fg->scaleShift, fg->compPresent, c->copyStream)) return rc;
   c->launches += 1 + nPl;
-  B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;       // the picture buffer is free once the grained copy exists
+  if (int rc = mark_read(c, buf, c->copyStream)) return rc;                                   // the picture buffer is free once the grained copy exists
   if (fmt == B200_OUT_16) {
     for (int k = 0; k < nPl; k++) if (int rc = copy_host(planes[k], gr.p[k], (size_t)g.stride[k] * (k ? g.height >> 1 : g.height) * 2, cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   } else {
@@ -600,7 +632,7 @@ B200_API int b200_frame_hash_async(b200_ctx* c, int slot, int method, uint8_t* d
   B200_CUDA(cudaMemsetAsync(acc, 0, 32, c->copyStream));
   if (int rc = launch_hash(c->planes(buf), c->g, method, acc, dig, c->copyStream)) return rc;
   c->launches += (c->g.chromaFormat ? 3 : 1) + 1;
-  B200_CUDA(cudaEventRecord(c->readDone[buf], c->copyStream)); c->readPending[buf] = 1;
+  if (int rc = mark_read(c, buf, c->copyStream)) return rc;
   if (int rc = copy_host(digest, dig, 12, cudaMemcpyDeviceToHost, c->copyStream)) return rc;
   B200_CUDA(cudaEventRecord(c->ticketEv[t], c->copyStream));
   return t;

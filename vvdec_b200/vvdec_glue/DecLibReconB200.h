@@ -119,6 +119,9 @@ class DecLibReconB200
   // explicit scaling lists: the reference's own table set (Quant::init -> setScalingListDec, Quant.cpp:386) in one contiguous buffer; a TU's table is addressed by its
   // offset in it (b200_tu::slOff).  TrQuant derives privately from Quant, so the glue keeps a Quant of its own for the tables
   std::unique_ptr<Quant> m_quant; bool m_useSL = false; const int* m_slBase = nullptr; size_t m_slCount = 0; const void* m_slReg = nullptr;
+  // Pinned pages that stay registered after their memory is freed keep the old physical pages: a later allocation at the same address would then be copied
+  // from / to those pages instead of its own.  The scaling tables are unregistered before they move or go away.
+  void unpinScaling() { if( m_slReg ) b200_host_unregister( const_cast<void*>( m_slReg ) ); m_slReg = nullptr; }
   void setSlOff( const CodingUnit& cu, b200_tu& t ) const
   {
     if( !( t.flags & B200_TU_SCALING ) ) return;
@@ -436,7 +439,7 @@ class DecLibReconB200
       m_quant->init( pic );
       m_slBase = m_quant->getDequantCoeff( 0, 0, 0 );
       m_slCount = (size_t) ( m_quant->getDequantCoeff( SCALING_LIST_NUM - 1, SCALING_LIST_SIZE_NUM - 1, SCALING_LIST_SIZE_NUM - 1 ) - m_slBase ) + 64 * 64;
-      if( m_slReg != m_slBase && !m_dryRun ) { if( b200_host_register( const_cast<int*>( m_slBase ), m_slCount * sizeof( int ) ) == 0 ) m_slReg = m_slBase; }
+      if( m_slReg != m_slBase && !m_dryRun ) { unpinScaling(); if( b200_host_register( const_cast<int*>( m_slBase ), m_slCount * sizeof( int ) ) == 0 ) m_slReg = m_slBase; }
     }
     m_doSao = sps.getUseSAO();
     m_doAlf = sps.getUseALF() && !AdaptiveLoopFilter::getAlfSkipPic( cs );
@@ -578,7 +581,7 @@ class DecLibReconB200
 
 public:
   DecLibReconB200() = default;
-  ~DecLibReconB200() = default;
+  ~DecLibReconB200() { unpinScaling(); }                  // before m_quant frees the tables: a registration must not outlive its memory
   CLASS_COPY_MOVE_DELETE( DecLibReconB200 )
 
   // DecLibRecon::create (DecLibRecon.cpp:127)
