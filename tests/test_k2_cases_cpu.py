@@ -87,7 +87,7 @@ def test_threshold_tiles_sit_on_their_threshold(name):
         if m == 3 and c["bd"] > 10: continue
         for kind in kinds_per_mode.get(m, ["luma"] + (["chroma"] if c["chroma"] else [])):
             assert all((m * 4 + k, kind, e, o) in hit for e in "lrtb" for o in (-1, 0, 1)), (m, k, kind)
-    # DMVR tiles: the search window is fast only when every list's luma and chroma origins are interior (k2_inter.cu :276-277).  Where all the other
+    # DMVR tiles: the search window is fast only when every list's luma and chroma origins are interior (k2_inter.cu dmvr_search).  Where all the other
     # conditions hold, the marked origin decides the path; in 4:2:0 the chroma condition is the stricter one (icx >= 4 needs ix >= 8), so a luma threshold
     # tile whose chroma origin is outside takes the slow path anyway: only the 4:0:0 cases make the luma DMVR thresholds path boundaries
     even = all(st % 2 == 0 for st in c["strides"][:3 if c["chroma"] else 1])

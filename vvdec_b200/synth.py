@@ -1296,7 +1296,7 @@ def _mc_phase_case(W):
 # ---- windows of a tile (k2_inter.cu): the integer reference position of its first sample, and the interior tests
 def mc_tile_windows(pu, l, tx=0, ty=0):
     """Integer reference positions of tile (tx, ty) of a PU for list l before any clipping: luma (ox, oy), chroma (ocx, ocy) as the uni / bi / BDOF tiles
-    compute them, and the DMVR search origins (ix, iy), (icx, icy) (mc_tile, :275 and :458)."""
+    compute them (mc_tile, motion per list), and the DMVR search origins (ix, iy), (icx, icy) (dmvr_search)."""
     bx, by = int(pu["x"]) + 16 * tx, int(pu["y"]) + 16 * ty
     mx, my = int(pu["mv"][l][0]), int(pu["mv"][l][1])
     return dict(luma=(bx + (mx >> 4), by + (my >> 4)), chroma=((bx >> 1) + (mx >> 5), (by >> 1) + (my >> 5)),
@@ -1304,8 +1304,8 @@ def mc_tile_windows(pu, l, tx=0, ty=0):
 
 
 def mc_window_margins(kind, W, H, tw, th):
-    """For a window kind, (first interior x, last interior x, first interior y, last interior y) of its origin: k2_inter.cu :472-473 (luma / chroma
-    footprints of the 8- / 4-tap filters) and :276-277 (DMVR search windows)."""
+    """For a window kind, (first interior x, last interior x, first interior y, last interior y) of its origin: the stage A predicates of k2_inter.cu
+    mc_tile (luma / chroma footprints of the 8- / 4-tap filters) and the search-window predicates of dmvr_search."""
     cw, ch, CW, CH = tw >> 1, th >> 1, W >> 1, H >> 1
     if kind == "luma": return 4, W - tw - 5, 3, H - th - 4
     if kind == "chroma": return 2, CW - cw - 3, 1, CH - ch - 2
@@ -1333,8 +1333,8 @@ def _mc_edge_specs(chroma, bd):
 def _mc_edges_case(W, H, ctu, chroma, bd):
     """Threshold tiles (see _mc_edge_specs), PUs with MVs at the clipMv bounds of this CTU size and one sample past them, and MVs near +-2^17.  The
     affine ones among the latter have sub-block MVs past the +-2^17 storage clamp.  The DMVR ones do not make the refinement cross that clamp
-    (k2_inter.cu :409): both search windows lie wholly outside the picture, where every sample replicates the border, so the search ends at the centre
-    with a zero delta.  No picture narrower than 2^13 samples can do otherwise, and clipMv follows the clamp in any case."""
+    (the clamp of the refined MV in k2_inter.cu dmvr_search): both search windows lie wholly outside the picture, where every sample replicates the
+    border, so the search ends at the centre with a zero delta.  No picture narrower than 2^13 samples can do otherwise, and clipMv follows the clamp in any case."""
     specs = _mc_edge_specs(chroma, bd)
     tools = ("uni0", "bi", "aff4_uni_prof") + (("dmvr_bdof",) if bd <= 10 else ())
     bounds = ("xlo", "xlo-1", "xhi", "xhi+1", "ylo", "ylo-1", "yhi", "yhi+1")
