@@ -255,16 +255,16 @@ static void pred_mip(const int16_t* src, int stride, int w, int h, int modeIdx, 
  * the CU has no left / above neighbour), xGetLMParameters :1694-1904 (up to four template positions, min / max pairs, a = diffC * DivSig >> y,
  * b, shift), predIntraChromaLM :519-539 (clip(((a * luma) >> shift) + b), Buffer.cpp:99 linTfCore).
  * T / L: the block's unfiltered chroma reference arrays (curChroma0 = getPredictorPtr).  luma: reconstructed luma plane. */
-static void pred_cclm(const b200_geom* g, const int16_t* luma, ptrdiff_t ls, const int16_t* src, int stride, const b200_intra_tu* t, int16_t* dst, ptrdiff_t ds)
+enum { CCLM_TS = 2 * 64 + 1 };
+/* the down-sampled luma (block and templates) into d0 (row -1 / column -1 hold the templates, row pitch CCLM_TS) and the parameters into p */
+static void cclm_derive(const b200_geom* g, const int16_t* luma, ptrdiff_t ls, const int16_t* src, int stride, const b200_intra_tu* t, int16_t* d0, orc_cclm* p)
 {
-  const int w = 1 << t->log2w, h = 1 << t->log2h, mode = t->mode, unit = 2, pmax = (1 << g->bitDepth) - 1;
+  const int w = 1 << t->log2w, h = 1 << t->log2h, mode = t->mode, unit = 2;
   const int aboveCu = (t->flags & B200_INTRA_LM_ABOVE) != 0, leftCu = (t->flags & B200_INTRA_LM_LEFT) != 0, colloc = (t->flags & B200_INTRA_LM_COLLOCATED) != 0;
   const int lx = t->x * 2, ly = t->y * 2;
   const int firstRowOfCtu = (ly & (g->ctuSize - 1)) == 0;
   const int16_t* rec = luma + (ptrdiff_t)ly * ls + lx;
-  enum { TS = 2 * 64 + 1 };
-  static _Thread_local int16_t tmp[(64 + 1) * TS + TS];
-  int16_t* d0 = tmp + TS + 1;                                       /* (0,0) of the block; row -1 / column -1 hold the template */
+  enum { TS = CCLM_TS };
   /* above template row */
   if (aboveCu) {
     /* the reference fills 2W samples for MDLM_T whatever exists there; only the lmAbove available units are ever read (:1770), so only those are made */
@@ -313,22 +313,37 @@ static void pred_cclm(const b200_geom* g, const int16_t* luma, ptrdiff_t ls, con
   if (sl[pmn[0]] > sl[pmx[1]]) { int* q = pmn; pmn = pmx; pmx = q; }
   if (sl[pmn[1]] > sl[pmx[0]]) { tt = pmn[1]; pmn[1] = pmx[0]; pmx[0] = tt; }
   const int minL = (sl[pmn[0]] + sl[pmn[1]] + 1) >> 1, minC = (sc[pmn[0]] + sc[pmn[1]] + 1) >> 1, maxL = (sl[pmx[0]] + sl[pmx[1]] + 1) >> 1, maxC = (sc[pmx[0]] + sc[pmx[1]] + 1) >> 1;
-  int a, b, shift;
+  int a, b, shift, normDiff = -1, clamped = 0;
   if (leftAvail || aboveAvail) {
     const int diff = maxL - minL;
     if (diff > 0) {
       static const uint8_t divSig[16] = {0, 7, 6, 5, 5, 4, 4, 3, 3, 2, 2, 1, 1, 1, 1, 0};
       const int diffC = maxC - minC;
       int x = ilog2(diff);
-      const int normDiff = (diff << 4 >> x) & 15, v = divSig[normDiff] | 8;
+      normDiff = (diff << 4 >> x) & 15;
+      const int v = divSig[normDiff] | 8;
       x += normDiff != 0;
       const int y = diffC == 0 ? 0 : ilog2(abs(diffC)) + 1, add = 1 << y >> 1;
       a = (diffC * v + add) >> y; shift = 3 + x - y;
-      if (shift < 1) { shift = 1; a = a == 0 ? 0 : a < 0 ? -15 : 15; }
+      if (shift < 1) { shift = 1; a = a == 0 ? 0 : a < 0 ? -15 : 15; clamped = 1; }
       b = minC - ((a * minL) >> shift);
     } else { a = 0; b = minC; shift = 0; }
   } else { a = 0; b = 1 << (g->bitDepth - 1); shift = 0; }
-  for (int j = 0; j < h; j++) for (int i = 0; i < w; i++) dst[j * ds + i] = (int16_t)iclip(0, pmax, ((a * d0[j * TS + i]) >> shift) + b);
+  p->a = a; p->b = b; p->shift = shift; p->minL = minL; p->maxL = maxL; p->minC = minC; p->maxC = maxC; p->cntT = cntT; p->cntL = cntL;
+  p->normDiff = normDiff; p->clamped = clamped;
+  for (int k = 0; k < 4; k++) { p->selL[k] = sl[k]; p->selC[k] = sc[k]; }
+  p->blkMin = 1 << 30; p->blkMax = -1;
+  for (int j = 0; j < h; j++) for (int i = 0; i < w; i++) { p->blkMin = imin(p->blkMin, d0[j * TS + i]); p->blkMax = imax(p->blkMax, d0[j * TS + i]); }
+}
+
+static void pred_cclm(const b200_geom* g, const int16_t* luma, ptrdiff_t ls, const int16_t* src, int stride, const b200_intra_tu* t, int16_t* dst, ptrdiff_t ds)
+{
+  static _Thread_local int16_t tmp[(64 + 1) * CCLM_TS + CCLM_TS];
+  int16_t* d0 = tmp + CCLM_TS + 1;                                  /* (0,0) of the block */
+  orc_cclm p;
+  cclm_derive(g, luma, ls, src, stride, t, d0, &p);
+  const int w = 1 << t->log2w, h = 1 << t->log2h, pmax = (1 << g->bitDepth) - 1;
+  for (int j = 0; j < h; j++) for (int i = 0; i < w; i++) dst[j * ds + i] = (int16_t)iclip(0, pmax, ((p.a * d0[j * CCLM_TS + i]) >> p.shift) + p.b);
 }
 
 static void pred_angular(const int16_t* src, int stride, int w0, int h0, int chroma, int dirMode, int mrl, int filtered, int doPDPC, int pmax, int16_t* dst, ptrdiff_t ds)
@@ -456,6 +471,17 @@ int orc_isp_tu_width(const b200_intra_tu* t)
   const int isp = isp_cu_of(t, &x0, &y0, &w, &h);
   if (isp == 2 && (w == 4 || (w == 8 && h > 4))) return imax(w >> 2, h < 16 ? 16 / h : 1);
   return 1 << t->log2w;
+}
+
+/* the parameters pred_cclm derives for a CCLM record (t->mode 70..72) over the planes as they are, without predicting */
+void orc_cclm_params(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* t, orc_cclm* out)
+{
+  const int w = 1 << t->log2w, h = 1 << t->log2h, stride = 2 * w + 1, rows = 2 * h + 1;
+  int16_t* ref = (int16_t*)calloc((size_t)stride * rows + 64, sizeof(int16_t));
+  static _Thread_local int16_t tmp[(64 + 1) * CCLM_TS + CCLM_TS];
+  fill_ref(planes[t->comp], g->stride[t->comp], t->x, t->y, w, h, 0, 2, 2, (t->flags & B200_INTRA_AVAIL_TL) ? 1 : 0, t->numAbove, t->numLeft, g->bitDepth, ref, stride);
+  cclm_derive(g, planes[0], g->stride[0], ref, stride, t, tmp + CCLM_TS + 1, out);
+  free(ref);
 }
 
 void orc_intra_tu(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* t)

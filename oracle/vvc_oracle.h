@@ -72,6 +72,11 @@ void orc_intra_predict(const b200_geom* g, int16_t* const planes[3], const b200_
 void orc_intra_isp_cu(const b200_geom* g, int16_t* luma, const int16_t* resi, int x0, int y0, int w, int h, int ispMode, int dirMode,
                       int availTL, int numAbove, int numLeft, int leftAvail, int aboveAvail, unsigned resiMask);
 void orc_intra_reconstruct(const b200_geom* g, int16_t* const planes[3], const int16_t* const resi[3], const b200_intra_tu* tus, size_t numTus);
+/* CCLM parameter derivation of one chroma record (xGetLMParameters): a, b, shift; the min / max luma and chroma averages; the four (luma, chroma)
+ * template pairs the min / max grouping sees (selL / selC, after the two-sample path duplicates its pair), cntT / cntL of them from the above / left
+ * template; normDiff (-1 without a slope) and whether shift < 1 clamped the slope; blkMin / blkMax: the range of the block's down-sampled luma.  Reads the planes as orc_intra_tu would at that point of a list. */
+typedef struct orc_cclm { int32_t a, b, shift, minL, maxL, minC, maxC, cntT, cntL, normDiff, clamped, selL[4], selC[4], blkMin, blkMax; } orc_cclm;
+void orc_cclm_params(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* t, orc_cclm* out);
 /* film grain synthesis, per-sample part (FilmGrainImpl::add_grain_block); tables as FilmGrainImpl holds them after FilmGrain::updateFGC:
  * pattern [2][8][64][64], sLUT / pLUT [3][256], lineSeeds [(h+15)/16] (FilmGrain::prepareBlockSeeds); 4:2:0, planes in place */
 void orc_film_grain(int16_t* const planes[3], const ptrdiff_t strides[3], int w, int h, int bitDepth, const int8_t* pattern, const uint8_t* sLUT,

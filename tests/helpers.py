@@ -12,6 +12,20 @@ i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
 i16p_off = C.c_void_p   # pointer into the middle of a buffer
 
 
+class Cclm(C.Structure):
+    """orc_cclm (oracle/vvc_oracle.h): what the oracle derives for one CCLM record."""
+    _fields_ = [(n, C.c_int32) for n in ("a", "b", "shift", "minL", "maxL", "minC", "maxC", "cntT", "cntL", "normDiff", "clamped")] + \
+               [("selL", C.c_int32 * 4), ("selC", C.c_int32 * 4), ("blkMin", C.c_int32), ("blkMax", C.c_int32)]
+
+
+def cclm_params(oracle, g, planes, rec):
+    """orc_cclm_params of one record (a numpy INTRA_TU_DTYPE scalar or row) over `planes`."""
+    r = np.array(rec, abi.INTRA_TU_DTYPE).reshape(1)
+    out = Cclm()
+    oracle.orc_cclm_params(C.byref(g), abi.plane_ptrs(planes), r.ctypes.data, C.byref(out))
+    return out
+
+
 def load_oracle():
     srcs = [os.path.join(ROOT, "oracle", f) for f in os.listdir(os.path.join(ROOT, "oracle")) if f.endswith((".c", ".h"))]
     if not os.path.exists(ORACLE_SO) or any(os.path.getmtime(s) > os.path.getmtime(ORACLE_SO) for s in srcs):
@@ -52,6 +66,7 @@ def load_oracle():
     lib.orc_intra_predict.argtypes = [C.POINTER(abi.Geom), PL, C.c_void_p, C.c_size_t]
     lib.orc_intra_isp_cu.argtypes = [C.POINTER(abi.Geom), i16p, C.c_void_p] + [C.c_int] * 11 + [C.c_uint]
     lib.orc_intra_reconstruct.argtypes = [C.POINTER(abi.Geom), PL, PL, C.c_void_p, C.c_size_t]
+    lib.orc_cclm_params.argtypes = [C.POINTER(abi.Geom), PL, C.c_void_p, C.POINTER(Cclm)]
     lib.orc_film_grain.argtypes = [PL, C.POINTER(C.c_ssize_t), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.orc_plane_hash.argtypes = [C.c_int, C.c_int, i16p, C.c_ssize_t, C.c_int, C.c_int, u8p]
     return lib
@@ -667,3 +682,32 @@ def lf_mismatch(oracle, case, got, want, dirs=3):
         return f"{case['name']}: plane {c}: {len(bad)} samples differ, first at (y={y}, x={x}): {a[y, x]} vs {b[y, x]}; written by: {seen or 'no classified segment'}"
     return None
 
+
+
+# ---- CCLM records the rules refuse (rules.cuh intra_problem), each row breaking one clause of a valid LM record; by default the picture is 256 x 256
+# with CTU 128, so a 64-wide or 64-high chroma block still fits one chroma CTU and only the CCLM clause refuses it (with a smaller CTU those rows are left out)
+def cclm_refusal_rows(W=256, H=256, ctu=128):
+    """(geometry, valid records, [(name, record, what b200_last_error() says)]): a valid 8x8 Cb / Cr LM block and the rows that break it."""
+    g = abi.make_geom(W, H, 10, ctu=ctu)
+    pw, ph = W // 2, H // 2
+    ok = np.zeros(2, abi.INTRA_TU_DTYPE)
+    for i, c in enumerate((1, 2)):
+        ok[i]["x"], ok[i]["y"], ok[i]["log2w"], ok[i]["log2h"], ok[i]["comp"], ok[i]["mode"] = 16, 16, 3, 3, c, abi.INTRA_LM
+        ok[i]["flags"] = abi.INTRA_AVAIL_TL | abi.INTRA_LM_ABOVE | abi.INTRA_LM_LEFT | abi.INTRA_ADD_RESI
+        ok[i]["numAbove"], ok[i]["numLeft"], ok[i]["lmAbove"], ok[i]["lmLeft"] = 8, 8, 4, 4
+
+    def row(name, what="bad CCLM block", **f):
+        r = ok[0].copy()
+        for k, v in f.items(): r[k] = v
+        return name, r, what
+    bare = dict(flags=0, numAbove=0, numLeft=0, lmAbove=0, lmLeft=0)
+    rows = [row("lm_on_luma", comp=0, x=32, y=32, **bare)]
+    if ctu == 128: rows += [row("chroma_64_wide", x=64, y=0, log2w=6, **bare), row("chroma_64_high", x=0, y=64, log2h=6, **bare)]
+    rows += [
+            row("lmAbove_over_w", lmAbove=9), row("lmLeft_over_h", lmLeft=9),
+            row("lm_above_at_y0", y=0, flags=abi.INTRA_LM_ABOVE, numAbove=0, numLeft=0, lmLeft=0),
+            row("lm_left_at_x0", x=0, flags=abi.INTRA_LM_LEFT, numAbove=0, numLeft=0, lmAbove=0),
+            row("template_past_right", mode=abi.INTRA_MDLM_T, x=pw - 8, lmAbove=8, numAbove=4),
+            row("template_past_bottom", mode=abi.INTRA_MDLM_L, y=ph - 8, lmLeft=8, numLeft=4),
+            row("mode_73", "bad mode", mode=73)]
+    return g, ok, rows

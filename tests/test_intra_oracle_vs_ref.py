@@ -12,9 +12,12 @@ pytestmark = pytest.mark.ref
 CHROMA_MODES = [0, 1, 18, 50, 2, 34, 66, 70, 70, 70, 23, 45, 61]       # 70 = DM (PU::getFinalIntraMode -> the luma mode)
 
 
-def run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, k, dirL, dirC, mrl, bdpcm, bdpcmC=0, mip=0, colloc=0):
+def run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, k, dirL, dirC, mrl, bdpcm, bdpcmC=0, mip=0, colloc=0, paint=None, out=None):
+    """paint(planes): writes designed neighbour samples into the noise planes before the reference runs; out: a list the reference's planes are
+    appended to."""
     g = abi.make_geom(W, H, bd, ctu=ctu)
     planes = synth.noise_planes(rng, W, H, bd)
+    if paint: paint(planes)
     cus = np.zeros(k + 1, synth.REF_INTRA_CU_DTYPE)
     for i in range(k + 1):
         cus[i]["x"], cus[i]["y"], cus[i]["w"], cus[i]["h"] = layout[i]
@@ -39,6 +42,7 @@ def run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, k, dirL, dirC, mrl, 
     mine = mine[-n:]
     for f in ("x", "y", "log2w", "log2h", "comp", "mode", "multiRefIdx", "flags", "numAbove", "numLeft", "mip", "lmAbove", "lmLeft"):
         assert np.array_equal(mine[f], recs[f]), (f, mine[f], recs[f], layout[k])
+    if out is not None: out.append(want)
     return recs
 
 
@@ -121,6 +125,39 @@ def test_intra_cclm(oracle, ref, w, h, colloc):
         for mode in (67, 68, 69):
             for rep in range(3):
                 run_case(oracle, ref, rng, W, H, 10 if rep else 8, ctu, rep & 1, layout, k, int(rng.integers(0, 67)), mode, 0, 0, colloc=colloc)
+
+
+@pytest.mark.parametrize("colloc", [0, 1])
+@pytest.mark.parametrize("bd,simd", [(8, 0), (8, 1), (10, 0), (10, 1), (12, 0)])
+def test_intra_cclm_designed(oracle, ref, bd, simd, colloc):
+    """CCLM on designed neighbour planes (synth.cclm_target_values painted as the GPU sweep paints them): every target of the parameter derivation
+    (every weak ordering of the four selected luma samples with distinct chroma, diff == 0, diffC == 0, each normDiff with either sign of diffC, the
+    slope clamped to +-15) with LM (two above + two left), MDLM_T (four above) and MDLM_L (four left), and the three orderings of the two-sample path;
+    the co-located luma is the reference's planar prediction over the designed rows and columns.  The 12-bit case runs the C kernels only (see
+    test_intra_random_layouts)."""
+    from tests.helpers import cclm_params
+    rng = np.random.default_rng(bd * 4 + simd * 2 + colloc)
+    W, H, ctu = 256, 256, 128
+    interior = ([(0, 0, 64, 64), (64, 0, 64, 64), (0, 64, 64, 64), (64, 64, 16, 16)], 3)
+    two = ([(0, 0, 64, 64), (64, 0, 16, 4)], 1)                      # top picture edge: 8x2 chroma with a left template of two samples
+    jobs = [(interior, dirC, t) for dirC in (67, 68, 69) for t in synth.CCLM_TARGETS if t[0] in ("tie", "diff0", "diffC0", "normDiff", "clamp")]
+    jobs += [(two, 67, ("tie2", o)) for o in range(3)]
+    reached = set()
+    for (layout, k), dirC, t in jobs:
+        mine = synth.gen_intra_records(rng, layout, W, H, modes={k: (0, dirC, 0, 0, 0)}, upto=k, colloc=colloc)[-2]
+        x, y, w, h = int(mine["x"]), int(mine["y"]), 1 << int(mine["log2w"]), 1 << int(mine["log2h"])
+        sel_l, sel_c = synth.cclm_target_values(t, bd)
+        want = []
+        recs = run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, k, 0, dirC, 0, 0, colloc=colloc, out=want,
+                        paint=lambda planes: synth.cclm_paint(planes, x, y, w, h, mine, sel_l, sel_c, bd))
+        p = cclm_params(oracle, abi.make_geom(W, H, bd, ctu=ctu), want[0], recs[1])
+        sl = list(p.selL)
+        got = {"tie": ("tie",) + tuple(sorted(set(sl)).index(v) for v in sl), "tie2": ("tie2", 0 if sl[1] < sl[0] else 1 if sl[1] == sl[0] else 2),
+               "diff0": ("diff0",) if p.maxL == p.minL else None, "diffC0": ("diffC0",) if p.maxC == p.minC and p.maxL > p.minL else None,
+               "normDiff": ("normDiff", p.normDiff, 1 if p.maxC > p.minC else -1), "clamp": ("clamp", 1 if p.a > 0 else -1) if p.clamped else None}[t[0]]
+        assert got == t, (dirC, t, got, sl)
+        reached.add((dirC, t))
+    assert len(reached) == len(jobs)
 
 
 @pytest.mark.parametrize("w,h", [(8, 8), (16, 16), (32, 32), (64, 64), (16, 8), (8, 16), (64, 16), (16, 64), (32, 8), (4, 16), (16, 4)])

@@ -1,8 +1,11 @@
 """The K6 test lists reach what tests/test_k6_intra_gpu.py claims they reach (no device needed): the designed sweep holds every block it lists and no
 block of it reads another, and the generated cases put more than 1024 records into one CTU, stay below the density threshold where they stand for a B
-picture, and never use MRL on the first row of a CTU."""
+picture, and never use MRL on the first row of a CTU.  The designed CCLM sweep reaches every geometry and parameter-derivation target it claims (as the
+oracle derives them), and the rules refuse each malformed CCLM record on the host."""
+import ctypes as C
 import numpy as np
 import pytest
+import vvdec_b200
 from vvdec_b200 import abi, synth
 from tests import helpers
 
@@ -88,3 +91,142 @@ def test_no_mrl_on_the_first_row_of_a_ctu(ctu):
         recs = synth.gen_intra_records(rng, layout, 416, 240, p_mrl=0.5, ctu=ctu)
         mrl = recs[recs["multiRefIdx"] > 0]
         assert len(mrl) > 20 and not (mrl["y"] % ctu == 0).any()
+
+
+# ---- the designed CCLM sweep (synth.cclm_sweep): what each case reaches, classified by the oracle's own derivation (orc_cclm_params)
+def _cclm_reached(p, bd):
+    """The targets (synth.CCLM_TARGETS, and ("tie2", order) on the two-sample path) one record reaches, and which selection it took."""
+    pmax, sl, n = (1 << bd) - 1, list(p.selL), p.cntT + p.cntL
+    out = set()
+    if n == 4: out.add(("tie",) + tuple(sorted(set(sl)).index(v) for v in sl))
+    if n == 2: out.add(("tie2", 0 if sl[1] < sl[0] else 1 if sl[1] == sl[0] else 2))   # the pair (s0, s1) comes back as s1, s0, s1, s0
+    if n and p.maxL == p.minL: out.add(("diff0",))
+    if p.maxL > p.minL and p.maxC == p.minC: out.add(("diffC0",))
+    if p.normDiff >= 0 and p.maxC != p.minC: out.add(("normDiff", p.normDiff, 1 if p.maxC > p.minC else -1))
+    if p.clamped and p.a: out.add(("clamp", 1 if p.a > 0 else -1))
+    ends = [((p.a * v) >> p.shift) + p.b for v in (p.blkMin, p.blkMax)]
+    if min(ends) < 0: out.add(("clip0",))
+    if max(ends) > pmax: out.add(("clipmax",))
+    if p.blkMin == 0: out.add(("luma0",))
+    if p.blkMax == pmax: out.add(("lumamax",))
+    sel = "2+2" if (p.cntT, p.cntL) == (2, 2) else "above" if p.cntT == 4 else "left" if p.cntL == 4 else "two" if n == 2 else "none"
+    return sel, out
+
+
+def _rules_accept(case):
+    g, recs = case["g"], case["recs"]
+    planes = [p.copy() for p in case["planes"]]
+    rc = vvdec_b200.lib().b200_intra_reconstruct(C.byref(g), abi.plane_ptrs(planes), abi.plane_ptrs(case["resi"]), recs.ctypes.data, len(recs))
+    assert rc in (0, -3), vvdec_b200.lib().b200_last_error()               # -3: no device (the host checks every record first)
+
+
+@pytest.mark.parametrize("name", [n for n in synth.CCLM_SWEEP_CASES if n.startswith("targets")])
+def test_cclm_targets_reached(oracle, name):
+    """Every target of the parameter derivation is reached with two above + two left, four above and four left, and the two-sample path takes its
+    three orderings; every block reaches what it was built for."""
+    case = synth.cclm_sweep(name)
+    g, bd = case["g"], case["bd"]
+    seen = {}
+    for r, tag in zip(case["recs"], case["tags"]):
+        sel, got = _cclm_reached(helpers.cclm_params(oracle, g, case["planes"], r), bd)
+        assert tag in got, (name, tag, sel, sorted(got), r)
+        seen.setdefault(sel, set()).update(got)
+    for sel in ("2+2", "above", "left"):
+        assert set(synth.CCLM_TARGETS) <= seen[sel], (sel, sorted(set(synth.CCLM_TARGETS) - seen[sel]))
+    assert {("tie2", o) for o in range(3)} <= seen["two"]
+    assert len([t for t in synth.CCLM_TARGETS if t[0] == "tie"]) == 75
+    _rules_accept(case)
+
+
+@pytest.mark.parametrize("name", [n for n in synth.CCLM_SWEEP_CASES if n.startswith("geometry")])
+def test_cclm_geometry_covered(name):
+    """Every chroma shape that fits the chroma CTU, with every LM / MDLM neighbourhood, under the 3-tap (first row of a CTU), 5-tap (collocated) and
+    6-tap filters; blocks without a left / above CU at the picture's left / top edge."""
+    case = synth.cclm_sweep(name)
+    recs, ctu, C = case["recs"], case["ctu"], case["ctu"] // 2
+    have = set()
+    for r in recs:
+        w, h, fl = 1 << int(r["log2w"]), 1 << int(r["log2h"]), int(r["flags"])
+        nb = (int(r["mode"]), int(bool(fl & abi.INTRA_LM_ABOVE)), int(bool(fl & abi.INTRA_LM_LEFT)), int(r["lmAbove"]), int(r["lmLeft"]), int(r["numAbove"]), int(r["numLeft"]))
+        first = bool(fl & abi.INTRA_LM_ABOVE) and (2 * int(r["y"])) % ctu == 0
+        have.add((w, h, nb, first, bool(fl & abi.INTRA_LM_COLLOCATED)))
+        if r["x"] == 0: have.add((w, h, "left_edge"))
+        if r["y"] == 0 and fl & abi.INTRA_LM_COLLOCATED: have.add((w, h, "top_edge"))
+    shapes = [(w, h) for (w, h) in synth.CCLM_SHAPES if w <= C and h <= C]
+    assert len(synth.CCLM_SHAPES) == 19 and (ctu < 64 or len(shapes) == 19)
+    for (w, h) in shapes:
+        nbs = synth.cclm_neighbourhoods(w, h)
+        for nb in nbs:
+            # the above template of a block as high as the chroma CTU always lies on the first row of a CTU (3-tap)
+            for first, colloc in [(h == C and bool(nb[1]), 0), (h == C and bool(nb[1]), 1)] + ([(True, 0), (True, 1)] if nb[1] else []):
+                if first and not colloc and (w, h, nb, True, True) in have and h < C: continue       # the first row is taken once, collocated or not
+                assert (w, h, nb, first, bool(colloc)) in have or (first and (w, h, nb, True, not colloc) in have), (w, h, nb, first, colloc)
+        assert (w, h, "left_edge") in have and (w, h, "top_edge") in have
+        for mode, k in ((abi.INTRA_MDLM_T, 3), (abi.INTRA_MDLM_L, 4)):
+            n, m = (w, h) if mode == abi.INTRA_MDLM_T else (h, w)
+            lm = {nb[k] for nb in nbs if nb[0] == mode}
+            assert {0, n // 2, n // 2 + min(n // 2, m // 2)} <= lm and len(lm) >= min(4, 2 + (min(n // 2, m // 2) >= 2))
+    _rules_accept(case)
+
+
+@pytest.mark.parametrize("name", [n for n in synth.CCLM_SWEEP_CASES if n != "chained"])
+def test_cclm_sweep_is_independent_and_in_ctu_order(name):
+    """No block's chroma reference samples (2w above incl. the corner, 2h left) are another block's samples, records are in CTU raster order, every
+    block inside its chroma CTU; the list holds chroma records only, so the luma every block reads is the planes' own."""
+    case = synth.cclm_sweep(name)
+    recs, W, ctu = case["recs"], case["W"], case["ctu"]
+    assert (recs["comp"] > 0).all() and (recs["mode"] >= abi.INTRA_LM).all()
+    key = ((recs["y"].astype(np.int64) * 2) // ctu) * (W // ctu) + (recs["x"].astype(np.int64) * 2) // ctu
+    assert np.all(np.diff(key) >= 0)
+    cs = ctu // 2
+    for c in (1, 2):
+        r = recs[recs["comp"] == c]
+        occ = np.zeros((case["H"] // 2, W // 2), bool)
+        for t in r:
+            x, y, w, h = int(t["x"]), int(t["y"]), 1 << int(t["log2w"]), 1 << int(t["log2h"])
+            assert x // cs == (x + w - 1) // cs and y // cs == (y + h - 1) // cs
+            assert not occ[y:y + h, x:x + w].any()
+            occ[y:y + h, x:x + w] = True
+        for t in r:
+            x, y, w, h = int(t["x"]), int(t["y"]), 1 << int(t["log2w"]), 1 << int(t["log2h"])
+            assert not occ[max(0, y - 1):y, max(0, x - 1):x + 2 * w].any() and not occ[max(0, y - 1):y + 2 * h, max(0, x - 1):x].any(), (c, x, y, w, h)
+
+
+def test_cclm_chained_depends_on_earlier_luma(oracle):
+    """The chained case: every CCLM block selects other template luma, and predicts something else in Cb or Cr, when the luma blocks before it are
+    left out; its templates come from luma blocks in the CTU above and in the CTU to the left."""
+    case = synth.cclm_sweep("chained")
+    g, recs, planes, ctu = case["g"], case["recs"], case["planes"], case["ctu"]
+    full = [p.copy() for p in planes]
+    oracle.orc_intra_predict(C.byref(g), abi.plane_ptrs(full), recs.ctypes.data, len(recs))
+    only = np.ascontiguousarray(recs[recs["comp"] > 0])
+    alone = [p.copy() for p in planes]
+    oracle.orc_intra_predict(C.byref(g), abi.plane_ptrs(alone), only.ctypes.data, len(only))
+    luma = np.ascontiguousarray(recs[recs["comp"] == 0])
+    lumad = [p.copy() for p in planes]
+    oracle.orc_intra_predict(C.byref(g), abi.plane_ptrs(lumad), luma.ctypes.data, len(luma))
+    assert len(only) >= 10
+    for t in only:
+        x, y, w, h = int(t["x"]), int(t["y"]), 1 << int(t["log2w"]), 1 << int(t["log2h"])
+        assert list(helpers.cclm_params(oracle, g, lumad, t).selL) != list(helpers.cclm_params(oracle, g, planes, t).selL), (x, y)
+        assert any(not np.array_equal(full[c][y:y + h, x:x + w], alone[c][y:y + h, x:x + w]) for c in (1, 2)), (x, y)
+        cx, cy = 2 * x // ctu, 2 * y // ctu
+        assert (((luma["x"] // ctu) == cx) & ((luma["y"] // ctu) == cy - 1)).any() and (((luma["x"] // ctu) == cx - 1) & ((luma["y"] // ctu) == cy)).any()
+    assert list(np.flatnonzero(recs["comp"] > 0)) != list(range(len(only)))   # luma records come first within each CTU
+    _rules_accept(case)
+
+
+@pytest.mark.parametrize("row", range(len(helpers.cclm_refusal_rows()[2])))
+def test_cclm_refusals_on_the_host(row):
+    """Each malformed CCLM record is refused before any device work, with the planes unchanged; the valid list is accepted."""
+    g, ok, rows = helpers.cclm_refusal_rows()
+    name, bad, what = rows[row]
+    lib = vvdec_b200.lib()
+    planes = [np.full((256 >> (c > 0), 256 >> (c > 0)), 100 + c, np.int16) for c in range(3)]
+    resi = [np.ones_like(p) for p in planes]
+    lst = np.ascontiguousarray(np.concatenate([ok, bad.reshape(1)]))
+    got = [p.copy() for p in planes]
+    assert lib.b200_intra_reconstruct(C.byref(g), abi.plane_ptrs(got), abi.plane_ptrs(resi), lst.ctypes.data, len(lst)) == -2, name
+    assert what.encode() in lib.b200_last_error(), (name, lib.b200_last_error())
+    assert all(np.array_equal(a, b) for a, b in zip(got, planes))
+    assert lib.b200_intra_reconstruct(C.byref(g), abi.plane_ptrs(got), abi.plane_ptrs(resi), ok.ctypes.data, len(ok)) in (0, -3)

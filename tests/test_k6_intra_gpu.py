@@ -102,7 +102,12 @@ def test_intra_predict_only_and_golden(b200):
 
 
 @functools.lru_cache(maxsize=None)
-def _sweep(reconstruct):
+def _sweep(reconstruct, name="modes"):
+    if name != "modes":                                           # a case of the designed CCLM sweep: its own planes and residual
+        case = synth.cclm_sweep(name)
+        g, planes, recs = case["g"], case["planes"], case["recs"]
+        resi = case["resi"] if reconstruct else None
+        return g, planes, resi, recs, _reconstruct(g, planes, resi, recs)
     W, H, recs = synth.intra_sweep()
     rng = np.random.default_rng(40)
     g = abi.make_geom(W, H, 10)
@@ -113,11 +118,15 @@ def _sweep(reconstruct):
 
 @pytest.mark.parametrize("kernel", INTRA_KERNELS)
 @pytest.mark.parametrize("reconstruct", [False, True], ids=["predict", "reconstruct"])
-def test_intra_designed_sweep(b200, kernel, reconstruct):
-    """Every (component, shape, mode) combination K6 takes, MRL, BDPCM and every MIP mode, each with a full, a partial and no neighbourhood, on noise
-    (tests/test_k6_cases_cpu.py checks that the list covers all of it and that no block reads another)."""
-    g, planes, resi, recs, want = _sweep(reconstruct)
-    assert_planes_equal(intra_run(b200, kernel, g, planes, recs, resi), want, kernel)
+@pytest.mark.parametrize("name", ["modes"] + list(synth.CCLM_SWEEP_CASES))
+def test_intra_designed_sweep(b200, kernel, reconstruct, name):
+    """modes: every (component, shape, mode) combination K6 takes, MRL, BDPCM and every MIP mode, each with a full, a partial and no neighbourhood, on
+    noise.  The CCLM cases (synth.CCLM_SWEEP_CASES): every chroma shape and LM / MDLM neighbourhood under each luma filter and at the picture edges;
+    templates designed to reach every target of the parameter derivation at 8, 10 and 12 bit; CCLM blocks whose templates and co-located luma are
+    written by luma blocks before them, in other CTUs.  tests/test_k6_cases_cpu.py checks what each list covers and that no block reads another
+    (except in the chained case)."""
+    g, planes, resi, recs, want = _sweep(reconstruct, name)
+    assert_planes_equal(intra_run(b200, kernel, g, planes, recs, resi), want, (name, kernel))
 
 
 @functools.lru_cache(maxsize=None)
@@ -179,3 +188,21 @@ def test_intra_ctu_block_limit(b200, kernel):
         assert rc == 0, b200.b200_last_error()
         assert_planes_equal(got, _reconstruct(g, planes, resi, many), kernel)
     assert_planes_equal(intra_run(b200, kernel, g, planes, recs, resi), want, kernel)
+
+
+@pytest.mark.parametrize("kernel", ("v1", "v2"))
+def test_intra_cclm_refusals(b200, kernel):
+    """Each malformed CCLM record (tests.helpers.cclm_refusal_rows: an LM mode on luma, 64-wide / 64-high chroma, lmAbove > w, lmLeft > h, LM_ABOVE at
+    y < 2, LM_LEFT at x < 2, a template past the right / bottom edge, mode 73) is refused with the planes unchanged, and the next valid list runs."""
+    g, ok, rows = helpers.cclm_refusal_rows()
+    rng = np.random.default_rng(43)
+    planes = synth.noise_planes(rng, g.width, g.height, g.bitDepth)
+    resi = [rng.integers(-40, 41, size=p.shape).astype(np.int16) for p in planes]
+    for name, bad, what in rows:
+        lst = np.ascontiguousarray(np.concatenate([ok, bad.reshape(1)]))
+        got = [p.copy() for p in planes]
+        with helpers.intra_kernel(kernel):
+            assert b200.b200_intra_reconstruct(C.byref(g), abi.plane_ptrs(got), abi.plane_ptrs(resi), lst.ctypes.data, len(lst)) == -2, name
+        assert what.encode() in b200.b200_last_error(), (name, b200.b200_last_error())
+        assert_planes_equal(got, planes, name)
+        assert_planes_equal(intra_run(b200, kernel, g, planes, ok, resi), _reconstruct(g, planes, resi, ok), (name, kernel))

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import vvdec_b200
 from vvdec_b200 import abi, synth
-from tests.helpers import oracle_decompress, intra_kernel
+from tests.helpers import oracle_decompress, intra_kernel, cclm_refusal_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -306,6 +306,16 @@ def test_intra_list_refusals(b200, oracle, kernel):
             with intra_kernel(kernel):
                 assert b200.b200_decompress_picture(ctx, C.byref(pic["struct"])) == -2 and b"intra block record" in b200.b200_last_error(), (comp, x, y)
             recs[i] = keep
+        # the CCLM rows of tests.helpers.cclm_refusal_rows for this picture (CTU 64: no 64-wide chroma rows), each in place of a chroma record: the
+        # device validator of the picture path refuses each
+        i = int(np.flatnonzero(recs["comp"] == 1)[0]); keep = recs[i].copy()
+        for name, bad, _ in cclm_refusal_rows(W, H, ctu)[2]:
+            recs[i] = bad
+            with intra_kernel(kernel):
+                h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"]))
+                rc = h if h < 0 else b200.b200_wait_picture(ctx, h, None, 0)
+            assert rc == -2 and b"intra block record" in b200.b200_last_error(), (name, rc, b200.b200_last_error())
+        recs[i] = keep
         decode_and_check()
 
         # one valid luma block repeated 3100 times, in the first CTU

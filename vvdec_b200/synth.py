@@ -1119,6 +1119,227 @@ def intra_record_key(r):
     return (int(r["comp"]), 1 << int(r["log2w"]), 1 << int(r["log2h"]), int(r["mode"]), int(r["multiRefIdx"]), int(r["mip"]))
 
 
+# ---------------------------------------------------------------------------------------------------------------- designed CCLM sweep
+# Chroma CCLM records (modes LM, MDLM_L, MDLM_T) over 4:2:0 planes, as named cases (tests/test_k6_*.py):
+#   geometry_ctu{32,64,128}: every chroma shape the reference codes with every LM / MDLM neighbourhood, under each luma down-sampling filter (3-tap on
+#     the first row of a CTU, 5-tap collocated, 6-tap), blocks without a left / above CU also at the picture's left / top edge; on noise.
+#   targets_{8,10,12}bit: 8x8 blocks whose templates are written so that the four selected (luma, chroma) pairs reach each target of the parameter
+#     derivation (CCLM_TARGETS) with both selections (two above + two left, four from one side), and 2-high blocks on the two-sample path.
+#   chained: luma blocks earlier in the list write the templates (in the CTUs above and to the left) and the co-located luma of the CCLM blocks.
+# Every block owns its footprint: the two chroma rows / columns in front of it and its 2w x 2h reference reach (the luma footprint is twice that).
+# Footprints never overlap, so no block reads another block's output (except in the chained case, on purpose) or another block's designed samples.
+CCLM_SHAPES = tuple((w, h) for w in (4, 8, 16, 32) for h in (2, 4, 8, 16, 32) if w * h >= 16)
+CCLM_WEAK_ORDERS = tuple(sorted({tuple(sorted(set(r)).index(v) for v in r) for r in np.ndindex(4, 4, 4, 4)}))      # the 75 weak orderings of 4 samples
+CCLM_TARGETS = (tuple(("tie",) + o for o in CCLM_WEAK_ORDERS) + (("diff0",), ("diffC0",)) + tuple(("normDiff", n, s) for n in range(16) for s in (1, -1))
+                + (("clamp", 1), ("clamp", -1), ("clip0",), ("clipmax",), ("luma0",), ("lumamax",)))
+CCLM_SWEEP_CASES = {
+    "geometry_ctu32": ("geometry", 32, 10), "geometry_ctu64": ("geometry", 64, 8), "geometry_ctu128": ("geometry", 128, 12),
+    "targets_8bit": ("targets", 128, 8), "targets_10bit": ("targets", 128, 10), "targets_12bit": ("targets", 128, 12),
+    "chained": ("chained", 64, 10),
+}
+
+
+def cclm_picks(num, alone):
+    """Template positions xGetLMParameters selects from `num` samples of one side: two, or four when the other side is absent (`alone`)."""
+    start, step = num >> (2 + alone), max(1, num >> (1 + alone))
+    return [start + k * step for k in range(min(num, (1 + alone) << 1))]
+
+
+def cclm_neighbourhoods(w, h):
+    """(mode, above, left, lmAbove, lmLeft, numAbove, numLeft) of every LM / MDLM neighbourhood of a w x h chroma block, consistent as the glue
+    flattener derives them (flatten_intra.h:102-112): LM with each (above, left) pair; MDLM_T with lmAbove at w/2, in between and at its largest
+    (w/2 + min(w/2, h/2) units, the above-right units available), and without an above CU; MDLM_L likewise."""
+    A = abi
+    out = [(A.INTRA_LM, a, l, w // 2 * a, h // 2 * l, w * a, h * l) for a in (1, 0) for l in (1, 0)]
+    for mode, n, m in ((A.INTRA_MDLM_T, w, h), (A.INTRA_MDLM_L, h, w)):
+        lo, hi = n // 2, n // 2 + min(n // 2, m // 2)
+        for v in sorted({lo, (lo + hi) // 2, hi}) + [0]:
+            side = (v, n // 2 + (v - lo if v else 0)) if v else (0, 0)            # (lm units, available units of 2n): the units beyond n are above-right / below-left
+            other = (m // 2, m)
+            if mode == A.INTRA_MDLM_T: out.append((mode, int(v > 0), 1, side[0], other[0], side[1], other[1]))
+            else: out.append((mode, 1, int(v > 0), other[0], side[0], other[1], side[1]))
+    return out
+
+
+def _cclm_record(x, y, w, h, comp, nb, colloc):
+    mode, above, left, lmA, lmL, numA, numL = nb
+    r = np.zeros((), abi.INTRA_TU_DTYPE)
+    r["x"], r["y"], r["log2w"], r["log2h"], r["comp"], r["mode"] = x, y, int(np.log2(w)), int(np.log2(h)), comp, mode
+    fl = abi.INTRA_ADD_RESI | (abi.INTRA_AVAIL_TL if above and left else 0) | (abi.INTRA_LM_ABOVE if above else 0) | (abi.INTRA_LM_LEFT if left else 0)
+    r["flags"] = fl | (abi.INTRA_LM_COLLOCATED if colloc else 0)
+    r["lmAbove"], r["lmLeft"], r["numAbove"], r["numLeft"] = lmA, lmL, numA, numL
+    return r
+
+
+def _cclm_pack(blocks, C, ctus_w):
+    """Chroma positions of blocks [(w, h, where)] in CTU raster order (size C, ctus_w CTUs a row): the first position on the 2-sample grid inside a
+    CTU where the block's footprint is free.  where: "any"; "first_row" (y on the first row of a CTU below the first); "left_edge" (x = 0); "top_edge" (y = 0)."""
+    Wc = C * ctus_w
+    occ = np.zeros((C * 128, Wc), bool)
+    cursor, out = {}, [None] * len(blocks)
+    for i in sorted(range(len(blocks)), key=lambda i: blocks[i][2] not in ("top_edge", "left_edge")):     # the edges first
+        w, h, where = blocks[i]
+        k = cursor.get((w, h, where), ctus_w if where == "first_row" else 0)
+        while True:
+            cx, cy = (k % ctus_w) * C, (k // ctus_w) * C
+            xs = [x for x in range(cx, cx + C - w + 1, 2) if x >= 2]
+            ys = [y for y in list(range(cy + 2, cy + C - h + 1, 2)) + [cy] if y >= 2]    # the first row of a CTU last: only a block as high as the CTU sits there
+            slots = [(x, y) for y in ys for x in xs]
+            cands = {"any": slots, "first_row": [(x, cy) for x in xs], "left_edge": [(0, y) for y in ys] if cx == 0 else [],
+                     "top_edge": [(x, 0) for x in xs] if cy == 0 else []}[where]
+            hit = next(((x, y) for (x, y) in cands if x + 2 * w <= Wc and not occ[max(0, y - 2):y + 2 * h, max(0, x - 2):x + 2 * w].any()), None)
+            if hit: break
+            k += 1
+            assert where != "top_edge" or k < ctus_w, "the top edge is full"
+        cursor[(w, h, where)] = k
+        x, y = hit
+        occ[max(0, y - 2):y + 2 * h, max(0, x - 2):x + 2 * w] = True
+        out[i] = hit
+    return out
+
+
+def cclm_paint(planes, x, y, w, h, rec, sel_l, sel_c, bd):
+    """Writes the templates of the CCLM record `rec` at chroma (x, y) so that the luma down-sampled at the selected positions (above ones first, as
+    xGetLMParameters takes them) is sel_l and the chroma there is sel_c (Cb; Cr gets pmax - sel_c), and the block's luma a ramp from 0 to pmax.  Luma
+    is written as constant cells: every tap of a selected position lies in that position's cell where selected positions are at least two apart."""
+    pmax = (1 << bd) - 1
+    Y, Cb, Cr = planes
+    mode, fl = int(rec["mode"]), int(rec["flags"])
+    above, left = bool(fl & abi.INTRA_LM_ABOVE), bool(fl & abi.INTRA_LM_LEFT)
+    top_n = 2 * int(rec["lmAbove"]) if mode == abi.INTRA_MDLM_T else w if mode == abi.INTRA_LM and above else 0
+    left_n = 2 * int(rec["lmLeft"]) if mode == abi.INTRA_MDLM_L else h if mode == abi.INTRA_LM and left else 0
+    pa = cclm_picks(top_n, int(not left_n)) if top_n else []
+    pl = cclm_picks(left_n, int(not top_n)) if left_n else []
+    assert len(pa) + len(pl) == len(sel_l)
+
+    def cell(picks, vals, i):                                       # the value of the first selected position at or after template position i
+        return next((v for p, v in zip(picks, vals) if p >= i), vals[-1])
+    lx, ly = 2 * x, 2 * y
+    for c in range(lx - 1, lx + 2 * top_n) if pa else ():            # rows above: position i reads columns 2i - 1 .. 2i + 1
+        Y[ly - 3:ly, c] = cell(pa, sel_l[:len(pa)], (c - lx) // 2)
+    for r in range(ly - 1, ly + 2 * left_n) if pl else ():           # columns left: position j reads rows 2j - 1 .. 2j + 1
+        Y[r, lx - 3:lx - (1 if r < ly else 0)] = cell(pl, sel_l[len(pa):], (r - ly) // 2)
+    ramp = np.clip(np.round((np.arange(2 * w) - w / 2) * pmax / w), 0, pmax)
+    Y[ly:ly + 2 * h, lx:lx + 2 * w] = ramp[None, :]
+    for p, v in zip(pa, sel_c[:len(pa)]): Cb[y - 1, x + p], Cr[y - 1, x + p] = v, pmax - v
+    for p, v in zip(pl, sel_c[len(pa):]): Cb[y + p, x - 1], Cr[y + p, x - 1] = v, pmax - v
+
+
+def cclm_target_values(t, bd, n=4):
+    """(sel_l, sel_c): template values that reach target t (a CCLM_TARGETS entry; the clip and luma targets ride on the clamped slopes) with n
+    selected samples (4, or 2 for the two-sample path, where t = ("tie2", order))."""
+    u, mid = 1 << (bd - 8), 1 << (bd - 1)
+    if t[0] == "tie2": return [mid - 40 * u + 40 * u * t[1], mid], [mid - 30 * u, mid + 50 * u]
+    if t[0] == "tie": return [mid - 60 * u + 40 * u * r for r in t[1:]], [mid - 60 * u, mid + 20 * u, mid - 20 * u, mid + 60 * u]
+    m, c = mid - 8 * u, mid + 3 * u
+    if t[0] == "diff0": return [m] * 4, [c - 30, c + 10, c - 10, c + 30]
+    if t[0] == "diffC0": return [m, m + 80 * u, m, m + 80 * u], [c] * 4
+    if t[0] == "normDiff": d, dc = 16 + t[1], 20 * t[2]
+    else: d, dc = 2, 100 * t[1]                                       # "clamp": diff 2, |diffC| 100: shift = 3 + 1 - 7 < 1
+    return [m, m + d, m, m + d], [c, c + dc, c, c + dc]
+
+
+def _cclm_geometry_blocks(C):
+    """(w, h, nb, colloc, where) of a geometry case: each neighbourhood of each shape that fits a chroma CTU of size C under each filter, and the
+    neighbourhoods without a left (above) CU once more at the picture's left (top) edge."""
+    out = []
+    for (w, h) in CCLM_SHAPES:
+        if w > C or h > C: continue
+        nbs = cclm_neighbourhoods(w, h)
+        for k, nb in enumerate(nbs):
+            out += [(w, h, nb, 0, "any"), (w, h, nb, 1, "any")]
+            if nb[1]: out.append((w, h, nb, k & 1, "first_row"))
+        out.append((w, h, nbs[1], 0, "left_edge"))                 # LM above only: m = 0 at i = 0
+        out.append((w, h, nbs[2], 1, "top_edge"))                  # LM left only, collocated: up = 0 at j = 0
+    return out
+
+
+def _cclm_target_blocks(bd):
+    """(w, h, nb, colloc, where, target, sel_l, sel_c) of a targets case: every target with two above + two left (LM), four above (LM above only /
+    MDLM_T) and four left (LM left only / MDLM_L), on 8x8 blocks; the three orderings of the two-sample path on 8x2, 16x2 and 32x2 (LM left only)."""
+    out = []
+    nbs = cclm_neighbourhoods(8, 8)
+    both, a_only, l_only = nbs[0], nbs[1], nbs[2]
+    mdlm_t = [nb for nb in nbs if nb[0] == abi.INTRA_MDLM_T][2]        # lmAbove at its largest
+    mdlm_l = [nb for nb in nbs if nb[0] == abi.INTRA_MDLM_L][2]
+    for k, t in enumerate(CCLM_TARGETS):
+        if t[0] in ("clip0", "clipmax", "luma0", "lumamax"): continue
+        sel_l, sel_c = cclm_target_values(t, bd)
+        for nb in (both, (a_only, mdlm_t)[k & 1], (l_only, mdlm_l)[k & 1]): out.append((8, 8, nb, k & 1, "any", t, sel_l, sel_c))
+    for w in (8, 16, 32):
+        for o in range(3):
+            sel_l, sel_c = cclm_target_values(("tie2", o), bd)
+            out.append((w, 2, cclm_neighbourhoods(w, 2)[2], 0, "any", ("tie2", o), sel_l, sel_c))
+    return out
+
+
+def _cclm_chained(ctu, bd, rng):
+    """CCLM blocks at the top-left corner of the CTUs of the second CTU row, each after the luma blocks that write its templates: a 32x8 block in the
+    CTU above (the above template), an 8x8 block in the CTU above-left (the corner), an 8x32 block in the CTU to the left (the left template) and the
+    co-located block; planar luma (a flat DC template would make the slope 0) over noise, so it differs from the noise the planes start with.  The
+    co-located block reads no neighbour, so it does not wait for the template blocks: only the CCLM block's own wait orders it after them."""
+    A = abi
+    n_ctu = 5
+    W, H = (n_ctu + 1) * ctu, 3 * ctu
+    luma, chroma = [], []
+    nbs = cclm_neighbourhoods(8, 8)
+    modes = [nbs[0], [nb for nb in nbs if nb[0] == A.INTRA_MDLM_T][2], [nb for nb in nbs if nb[0] == A.INTRA_MDLM_L][2], nbs[0], nbs[0]]
+    for k in range(n_ctu):
+        X = (k + 1) * ctu
+        for (lx, ly, w, h) in ((X - 8, ctu - 8, 8, 8), (X, ctu - 8, 32, 8), (X - 8, ctu, 8, 32), (X, ctu, 16, 16)):
+            r = np.zeros((), A.INTRA_TU_DTYPE)
+            r["x"], r["y"], r["log2w"], r["log2h"], r["mode"] = lx, ly, int(np.log2(w)), int(np.log2(h)), 0
+            if ly < ctu or lx < X:                                     # the template blocks; the co-located block has no neighbourhood of its own
+                r["numAbove"], r["numLeft"] = 2 * w // 4, 2 * h // 4
+                r["flags"] = A.INTRA_AVAIL_TL | (A.INTRA_FILTER_REF if intra_filter_ref(w, h, 0, 0, 0) else 0)
+            r["flags"] |= A.INTRA_ADD_RESI
+            luma.append(r)
+        for comp in (1, 2): chroma.append(_cclm_record(X // 2, ctu // 2, 8, 8, comp, modes[k], k & 1))
+    recs = np.array(luma + chroma, A.INTRA_TU_DTYPE)
+    key = ((recs["y"].astype(int) << (recs["comp"] > 0)) // ctu) * (W // ctu) + ((recs["x"].astype(int) << (recs["comp"] > 0)) // ctu)
+    return W, H, recs[np.argsort(key, kind="stable")], ["chained"] * len(recs)
+
+
+_cclm_sweep_cache = {}
+
+
+def cclm_sweep(name):
+    """One case of the designed CCLM sweep (CCLM_SWEEP_CASES) as a dict: geometry (g, W, H, bd, ctu), noise planes with the designed templates
+    written in (planes), the residual planes (resi), the records in CTU order (recs, Cb and Cr of each block) and per record what it was built for
+    (tags: the neighbourhood / filter / edge of a geometry block, the target of a targets block, Cr's with the chroma slope negated)."""
+    if name in _cclm_sweep_cache: return _cclm_sweep_cache[name]
+    kind, ctu, bd = CCLM_SWEEP_CASES[name]
+    rng = np.random.default_rng(sum(map(ord, name)))
+    C = ctu // 2
+    if kind == "chained":
+        W, H, recs, tags = _cclm_chained(ctu, bd, rng)
+        planes = noise_planes(rng, W, H, bd)
+    else:
+        blocks = _cclm_geometry_blocks(C) if kind == "geometry" else _cclm_target_blocks(bd)
+        ctus_w = max(8, 1024 // C)
+        pos = _cclm_pack([(b[0], b[1], b[4]) for b in blocks], C, ctus_w)
+        W = ctus_w * ctu
+        H = ((max(y + 2 * b[1] for (x, y), b in zip(pos, blocks)) + C - 1) // C + 1) * ctu
+        planes = noise_planes(rng, W, H, bd)
+        per = []
+        for (x, y), b in zip(pos, blocks):
+            w, h, nb, colloc, where = b[:5]
+            tag = ("geometry", nb, colloc, where) if kind == "geometry" else b[5]
+            rs = [_cclm_record(x, y, w, h, comp, nb, colloc) for comp in (1, 2)]
+            if kind == "targets": cclm_paint(planes, x, y, w, h, rs[0], b[6], b[7], bd)
+            neg = (tag[0], tag[1], -tag[2]) if tag[0] == "normDiff" else (tag[0], -tag[1]) if tag[0] == "clamp" else tag
+            per += [(rs[0], tag), (rs[1], neg)]
+        key = [((int(r["y"]) * 2) // ctu) * (W // ctu) + (int(r["x"]) * 2) // ctu for r, _ in per]
+        order = np.argsort(key, kind="stable")
+        recs = np.array([per[i][0] for i in order], abi.INTRA_TU_DTYPE)
+        tags = [per[i][1] for i in order]
+    g = abi.make_geom(W, H, bd, ctu=ctu)
+    resi = [rng.integers(-64, 65, size=p.shape).astype(np.int16) for p in planes]
+    case = dict(name=name, g=g, W=W, H=H, bd=bd, ctu=ctu, planes=planes, resi=resi, recs=recs, tags=tags)
+    _cclm_sweep_cache[name] = case
+    return case
+
+
 # ---------------------------------------------------------------------------------------------------------------- designed K2 sweep
 # A fixed list of named K2 cases (tests/test_k2_*.py): every PU shape under every tool it allows, every 1/16 luma phase pair in each tile list, tiles whose
 # reference windows sit on the interior / boundary thresholds of k2_inter.cu, MVs at the clipMv bounds and at +-2^17, and reference content built so that
