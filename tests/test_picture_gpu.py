@@ -584,3 +584,40 @@ def test_k1_lmcs_chroma_scaling_in_a_picture(b200, oracle, ctu):
             assert len(bad) == 0, f"CTU {ctu}: plane {c}: {len(bad)} diffs, first at {bad[:1].tolist()}"
     finally:
         b200.b200_ctx_destroy(ctx)
+
+
+def test_slice_map_without_deblocking_in_a_reused_arena(b200, oracle):
+    """A picture of several slices with deblocking off still carries its CTU slice map (the glue passes one whenever there is more than one slice); the
+    map is only read by deblocking, so it is neither uploaded nor checked.  The picture runs in the one arena right after a picture with the same work
+    lists and deblocking on: where its map entry lies, the arena still holds that picture's vertical edge grid, bytes far past the slice count.  It
+    decodes and equals the oracle chain's frame."""
+    W, H, bd = 416, 240, 10
+    g = abi.make_geom(W, H, bd)
+    rng = np.random.default_rng(12)
+    refs = [synth.noise_planes(rng, W, H, bd) for _ in range(4)]
+    nctu = ((W + 127) // 128) * ((H + 127) // 128)
+    first = synth.gen_picture(rng, W, H, bd, dst_slot=4, sao=False, alf=False)
+    first["lfSlices"] = np.zeros(4, synth.LFSLICE_DTYPE); first["ctuSlice"] = (np.arange(nctu) % 4).astype(np.uint8)
+    st = first["struct"]; st.lfSlices = first["lfSlices"].ctypes.data; st.numLfSlices = 4; st.ctuSlice = first["ctuSlice"].ctypes.data
+    # the same lists without deblocking: the two grid entries shrink to 256 bytes each, so the map entry starts 512 bytes into the first picture's lfV
+    assert first["lfV"].reshape(-1).view(np.uint8)[512:512 + nctu].max() >= 2
+    second = {k: first[k] for k in ("pus", "ndmvr", "tus", "coefs")}
+    second["sao"] = synth.gen_sao(rng, W, H, 128, bd, p_on=0.5)
+    second["ctuSlice"] = (np.arange(nctu) % 2).astype(np.uint8); second["lfSlices"] = np.zeros(2, synth.LFSLICE_DTYPE)
+    st = abi.Picture.from_buffer_copy(st); second["struct"] = st
+    st.dstSlot = 5; st.flags = abi.PIC_SAO; st.sao = second["sao"].ctypes.data
+    st.ctuSlice = second["ctuSlice"].ctypes.data; st.lfSlices = second["lfSlices"].ctypes.data; st.numLfSlices = 2
+    want, _ = oracle_decompress(oracle, g, refs, second)
+    ctx = C.c_void_p()
+    vvdec_b200.check(b200.b200_ctx_create(C.byref(ctx), C.byref(g), 6, 1, -1))
+    try:
+        for s in range(4): vvdec_b200.check(b200.b200_ctx_load_slot(ctx, s, abi.plane_ptrs(refs[s])))
+        for pic in (first, second):
+            h = b200.b200_decompress_picture(ctx, C.byref(pic["struct"]))
+            assert h == 0, b200.b200_last_error()
+            vvdec_b200.check(b200.b200_wait_picture(ctx, h, None, 0))
+        got = [np.zeros_like(p) for p in want]
+        vvdec_b200.check(b200.b200_get_frame(ctx, 5, abi.plane_ptrs(got)))
+        for c in range(3): assert np.array_equal(got[c], want[c]), f"plane {c}"
+    finally:
+        b200.b200_ctx_destroy(ctx)

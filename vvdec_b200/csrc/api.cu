@@ -31,35 +31,19 @@ int ensure_device()
   return status;
 }
 
-// scratch for the kernel-level host wrappers (single-threaded use, like the reference's per-thread objects)
+// scratch for the kernel-level host wrappers (single-threaded use, like the reference's per-thread objects): one buffer, laid out per call by a Staging plan
 struct HostWrapScratch {
-  DevBuf planes[3], tus, coefs, scaling, misc[8];
+  DevBuf buf;
   cudaStream_t stream = nullptr;
   int init() { if (!stream) { B200_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking)); } return 0; }
 };
 static HostWrapScratch g_hw;
 HostWrapScratch& host_scratch() { return g_hw; }
 
-// Upload the three host planes described by g into scratch; fills dp.
-static int upload_planes(const b200_geom* g, int16_t* const planes[3], DevPlanes& dp, cudaStream_t s)
-{
-  const int nPlanes = g->chromaFormat ? 3 : 1;
-  for (int c = 0; c < nPlanes; c++) {
-    const int ph = c ? g->height >> 1 : g->height;
-    const size_t bytes = (size_t)g->stride[c] * ph * sizeof(int16_t);
-    if (int rc = g_hw.planes[c].reserve(bytes)) return rc;
-    dp.p[c] = g_hw.planes[c].as<int16_t>(); dp.stride[c] = g->stride[c];
-    B200_CUDA(cudaMemcpyAsync(dp.p[c], planes[c], bytes, cudaMemcpyHostToDevice, s));
-  }
-  return 0;
-}
+// whole planes (strides, padding included) of dp back to the caller's planes
 static int download_planes(const b200_geom* g, int16_t* const planes[3], const DevPlanes& dp, cudaStream_t s)
 {
-  const int nPlanes = g->chromaFormat ? 3 : 1;
-  for (int c = 0; c < nPlanes; c++) {
-    const int ph = c ? g->height >> 1 : g->height;
-    B200_CUDA(cudaMemcpyAsync(planes[c], dp.p[c], (size_t)g->stride[c] * ph * sizeof(int16_t), cudaMemcpyDeviceToHost, s));
-  }
+  for (int c = 0; c < (g->chromaFormat ? 3 : 1); c++) B200_CUDA(cudaMemcpyAsync(planes[c], dp.p[c], plane_bytes(*g, c), cudaMemcpyDeviceToHost, s));
   return 0;
 }
 
@@ -119,16 +103,11 @@ B200_API int b200_k1_residual(const b200_geom* g, int16_t* const planes[3], cons
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
   K1Launch L; L.geom = *g; L.numTus = numTus; L.mode = mode;
-  if (int rc = upload_planes(g, planes, L.planes, s)) return rc;
-  if (int rc = g_hw.tus.reserve(numTus * sizeof(b200_tu))) return rc;
-  if (int rc = g_hw.coefs.reserve(numCoefs * sizeof(int16_t) + 16)) return rc;
-  if (int rc = g_hw.scaling.reserve(numScaling * sizeof(int32_t) + 16)) return rc;
-  if (int rc = g_hw.misc[4].reserve(numTus * 4 + LM_INTS * sizeof(int) + 256)) return rc;
-  if (numTus) B200_CUDA(cudaMemcpyAsync(g_hw.tus.p, tus, numTus * sizeof(b200_tu), cudaMemcpyHostToDevice, s));
-  if (numCoefs) B200_CUDA(cudaMemcpyAsync(g_hw.coefs.p, coefs, numCoefs * sizeof(int16_t), cudaMemcpyHostToDevice, s));
-  if (numScaling) B200_CUDA(cudaMemcpyAsync(g_hw.scaling.p, scaling, numScaling * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  L.tus = g_hw.tus.as<b200_tu>(); L.coefs = g_hw.coefs.as<int16_t>(); L.scaling = g_hw.scaling.as<int32_t>();
-  int* meta = g_hw.misc[4].as<int>(); uint32_t* idx = reinterpret_cast<uint32_t*>(meta + LM_INTS);
+  int* meta; uint32_t* idx;
+  Staging st;
+  stage_picture(st, L.planes, planes, *g); st.add(&L.tus, tus, numTus); st.add(&L.coefs, coefs, numCoefs); st.add(&L.scaling, scaling, numScaling);
+  st.add(&meta, nullptr, LM_INTS); st.add(&idx, nullptr, numTus);
+  if (int rc = st.commit(g_hw.buf, s)) return rc;
   if (int rc = launch_tu_bucket(L.tus, numTus, idx, meta, *g, numCoefs, numScaling, s)) return rc;
   L.idx = idx; L.meta = meta;
   if (int rc = fetch_list_meta(meta, L.cnt, K1_LISTS, "b200_k1_residual", s)) return rc;
@@ -158,17 +137,10 @@ B200_API int b200_lf_deblock(const b200_geom* g, int16_t* const planes[3], const
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
   LfLaunch L; L.geom = *g; L.dirs = dirs;
-  memset(&L.slices, 0, sizeof(L.slices)); memcpy(L.slices.s, slices, numSlices * sizeof(b200_lf_slice));
-  if (seq) L.seq = *seq; else memset(&L.seq, 0, sizeof(L.seq));
-  if (int rc = upload_planes(g, planes, L.planes, s)) return rc;
-  if (int rc = g_hw.misc[0].reserve(n4 * sizeof(b200_lf_param))) return rc;
-  if (int rc = g_hw.misc[1].reserve(n4 * sizeof(b200_lf_param))) return rc;
-  if (int rc = g_hw.misc[2].reserve(nCtu)) return rc;
-  B200_CUDA(cudaMemcpyAsync(g_hw.misc[0].p, lfV, n4 * sizeof(b200_lf_param), cudaMemcpyHostToDevice, s));
-  B200_CUDA(cudaMemcpyAsync(g_hw.misc[1].p, lfH, n4 * sizeof(b200_lf_param), cudaMemcpyHostToDevice, s));
-  if (ctuSlice) B200_CUDA(cudaMemcpyAsync(g_hw.misc[2].p, ctuSlice, nCtu, cudaMemcpyHostToDevice, s));
-  L.lfV = g_hw.misc[0].as<b200_lf_param>(); L.lfH = g_hw.misc[1].as<b200_lf_param>();
-  L.ctuSlice = ctuSlice ? g_hw.misc[2].as<uint8_t>() : nullptr;
+  lf_tables(L, slices, numSlices, seq);
+  Staging st;
+  stage_picture(st, L.planes, planes, *g); st.add(&L.lfV, lfV, n4); st.add(&L.lfH, lfH, n4); st.add(&L.ctuSlice, ctuSlice, ctuSlice ? nCtu : 0);
+  if (int rc = st.commit(g_hw.buf, s)) return rc;
   if (int rc = launch_lf_deblock(L, s)) return rc;
   if (int rc = download_planes(g, planes, L.planes, s)) return rc;
   B200_CUDA(cudaStreamSynchronize(s));
@@ -185,20 +157,6 @@ static int download_plane_rows(const b200_geom* g, int16_t* const planes[3], con
   return 0;
 }
 
-static int upload_src_alloc_dst(const b200_geom* g, const int16_t* const src[3], DevPlanes& ds, DevPlanes& dd, cudaStream_t s)
-{
-  const int nPlanes = g->chromaFormat ? 3 : 1;
-  for (int c = 0; c < nPlanes; c++) {
-    const int ph = c ? g->height >> 1 : g->height;
-    const size_t bytes = (size_t)g->stride[c] * ph * sizeof(int16_t);
-    if (int rc = g_hw.planes[c].reserve(bytes)) return rc;
-    if (int rc = g_hw.misc[3 + c].reserve(bytes)) return rc;
-    ds.p[c] = g_hw.planes[c].as<int16_t>(); dd.p[c] = g_hw.misc[3 + c].as<int16_t>(); ds.stride[c] = dd.stride[c] = g->stride[c];
-    B200_CUDA(cudaMemcpyAsync(ds.p[c], src[c], bytes, cudaMemcpyHostToDevice, s));
-  }
-  return 0;
-}
-
 B200_API int b200_sao_picture(const b200_geom* g, const int16_t* const src[3], int16_t* const dst[3], const b200_sao_ctu* ctus, const b200_vb* vb)
 {
   B200_CHECK(g && src && dst && ctus, "b200_sao_picture: null argument");
@@ -211,11 +169,9 @@ B200_API int b200_sao_picture(const b200_geom* g, const int16_t* const src[3], i
   cudaStream_t s = g_hw.stream;
   SaoLaunch L; L.geom = *g;
   if (vb) L.vb = *vb; else memset(&L.vb, 0, sizeof(L.vb));
-  if (int rc = upload_src_alloc_dst(g, src, L.src, L.dst, s)) return rc;
-  const size_t nCtu = (size_t)cl.ctusW * cl.ctusH;
-  if (int rc = g_hw.misc[0].reserve(nCtu * sizeof(b200_sao_ctu))) return rc;
-  B200_CUDA(cudaMemcpyAsync(g_hw.misc[0].p, ctus, nCtu * sizeof(b200_sao_ctu), cudaMemcpyHostToDevice, s));
-  L.ctus = g_hw.misc[0].as<b200_sao_ctu>();
+  Staging st;
+  stage_picture(st, L.src, src, *g); stage_picture(st, L.dst, nullptr, *g); st.add(&L.ctus, ctus, (size_t)cl.ctusW * cl.ctusH);
+  if (int rc = st.commit(g_hw.buf, s)) return rc;
   if (int rc = launch_sao(L, s)) return rc;
   if (int rc = download_plane_rows(g, dst, L.dst, s)) return rc;
   B200_CUDA(cudaStreamSynchronize(s));
@@ -233,26 +189,13 @@ B200_API int b200_intra_reconstruct(const b200_geom* g, int16_t* const planes[3]
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
   IntraLaunch L; L.geom = *g; L.numTus = numTus;
-  if (int rc = upload_planes(g, planes, L.planes, s)) return rc;
-  for (int c = 0; c < 3; c++) {
-    L.resi[c] = nullptr; L.owner[c] = nullptr; L.ownerStride[c] = 0; L.ownerBytes[c] = 0;
-    if (c >= nPl) continue;
-    const int pw = c ? g->width >> 1 : g->width, ph = c ? g->height >> 1 : g->height, unit = c ? 2 : 4;
-    L.ownerStride[c] = (pw + unit - 1) / unit; L.ownerBytes[c] = (size_t)L.ownerStride[c] * ((ph + unit - 1) / unit) * sizeof(int);
-    if (int rc = g_hw.misc[c].reserve(L.ownerBytes[c])) return rc;
-    L.owner[c] = g_hw.misc[c].as<int>();
-    if (resi && resi[c]) {
-      const size_t bytes = (size_t)g->stride[c] * ph * sizeof(int16_t);
-      if (int rc = g_hw.misc[3 + c].reserve(bytes)) return rc;
-      B200_CUDA(cudaMemcpyAsync(g_hw.misc[3 + c].p, resi[c], bytes, cudaMemcpyHostToDevice, s));
-      L.resi[c] = g_hw.misc[3 + c].as<int16_t>();
-    }
-  }
-  if (int rc = g_hw.tus.reserve(numTus * sizeof(b200_intra_tu) + 16)) return rc;
-  if (int rc = g_hw.misc[6].reserve((numTus + 2) * sizeof(int))) return rc;
-  if (int rc = g_hw.misc[7].reserve(intra_order_ints(*g, numTus) * sizeof(int))) return rc;
-  if (numTus) B200_CUDA(cudaMemcpyAsync(g_hw.tus.p, tus, numTus * sizeof(b200_intra_tu), cudaMemcpyHostToDevice, s));
-  L.tus = g_hw.tus.as<b200_intra_tu>(); L.sync = g_hw.misc[6].as<int>(); L.order = g_hw.misc[7].as<int>();
+  intra_owner_maps(L);
+  Staging st;
+  stage_picture(st, L.planes, planes, *g);
+  for (int c = 0; c < 3; c++) st.add(&L.resi[c], resi ? resi[c] : nullptr, c < nPl && resi && resi[c] ? plane_bytes(*g, c) / 2 : 0);
+  for (int c = 0; c < nPl; c++) st.add(&L.owner[c], nullptr, L.ownerBytes[c] / sizeof(int));
+  st.add(&L.tus, tus, numTus); st.add(&L.sync, nullptr, numTus + 2); st.add(&L.order, nullptr, intra_order_ints(*g, numTus));
+  if (int rc = st.commit(g_hw.buf, s)) return rc;
   if (int rc = launch_intra(L, s)) return rc;
   int err = 0;
   if (numTus) B200_CUDA(cudaMemcpyAsync(&err, L.sync + numTus + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -280,23 +223,9 @@ B200_API int b200_alf_picture(const b200_geom* g, const int16_t* const src[3], i
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
   AlfLaunch L; L.geom = *g;
-  if (int rc = upload_src_alloc_dst(g, src, L.src, L.dst, s)) return rc;
-  const size_t nCtu = (size_t)cl.ctusW * cl.ctusH;
-  const size_t nL = (size_t)T->numLumaSets * 1300, nC = (size_t)T->numChromaAlts * 7, n0 = (size_t)T->numCc[0] * 7, n1 = (size_t)T->numCc[1] * 7;
-  const size_t tabElems = 2 * nL + 2 * nC + n0 + n1 + 8;
-  if (int rc = g_hw.misc[0].reserve(nCtu * sizeof(b200_alf_ctu))) return rc;
-  if (int rc = g_hw.misc[1].reserve(tabElems * sizeof(int16_t))) return rc;
-  B200_CUDA(cudaMemcpyAsync(g_hw.misc[0].p, ctus, nCtu * sizeof(b200_alf_ctu), cudaMemcpyHostToDevice, s));
-  int16_t* d = g_hw.misc[1].as<int16_t>();
-  auto up = [&](const int16_t* h, size_t n, const int16_t*& out) -> int {
-    out = d; if (n) B200_CUDA(cudaMemcpyAsync(d, h, n * sizeof(int16_t), cudaMemcpyHostToDevice, s)); d += n; return 0; };
-  if (int rc = up(T->lumaCoeff, nL, L.lumaCoeff)) return rc;
-  if (int rc = up(T->lumaClip, nL, L.lumaClip)) return rc;
-  if (int rc = up(T->chromaCoeff, nC, L.chromaCoeff)) return rc;
-  if (int rc = up(T->chromaClip, nC, L.chromaClip)) return rc;
-  if (int rc = up(T->ccCoeff[0], n0, L.cc[0])) return rc;
-  if (int rc = up(T->ccCoeff[1], n1, L.cc[1])) return rc;
-  L.ctus = g_hw.misc[0].as<b200_alf_ctu>();
+  Staging st;
+  stage_picture(st, L.src, src, *g); stage_picture(st, L.dst, nullptr, *g); st.add(&L.ctus, ctus, (size_t)cl.ctusW * cl.ctusH); stage_alf_tables(st, L, T);
+  if (int rc = st.commit(g_hw.buf, s)) return rc;
   StreamSet ss(s);
   if (int rc = launch_alf(L, ss)) return rc;
   if (int rc = download_plane_rows(g, dst, L.dst, s)) return rc;
@@ -324,43 +253,23 @@ B200_API int b200_mc_predict_wp(const b200_geom* g, int16_t* const dst[3], const
   if (int rc = g_hw.init()) return rc;
   cudaStream_t s = g_hw.stream;
   McLaunch L; L.geom = *g;
-  if (int rc = upload_planes(g, dst, L.dst, s)) return rc;
-  const int nPlanes = g->chromaFormat ? 3 : 1;
-  size_t planeBytes[3] = {0, 0, 0}, total = 0;
-  for (int c = 0; c < nPlanes; c++) { planeBytes[c] = (((size_t)g->stride[c] * (c ? g->height >> 1 : g->height) * 2) + 255) & ~(size_t)255; total += planeBytes[c]; }
-  if (int rc = g_hw.misc[3].reserve(total * numSlots)) return rc;
-  std::vector<const int16_t*> ptrs(numSlots * 3, nullptr);
-  char* base = g_hw.misc[3].as<char>();
-  for (int sl = 0; sl < numSlots; sl++) {
-    size_t off = 0;
-    for (int c = 0; c < nPlanes; c++) {
-      char* d = base + (size_t)sl * total + off;
-      B200_CUDA(cudaMemcpyAsync(d, refs[sl * 3 + c], (size_t)g->stride[c] * (c ? g->height >> 1 : g->height) * 2, cudaMemcpyHostToDevice, s));
-      ptrs[sl * 3 + c] = reinterpret_cast<const int16_t*>(d); off += planeBytes[c];
-    }
-  }
   const size_t capTiles = mc_tile_capacity(*g, numPus);
-  if (int rc = g_hw.misc[5].reserve(numPus * sizeof(b200_pu) + 64)) return rc;
-  if (int rc = g_hw.misc[6].reserve(capTiles * 4 + LM_INTS * sizeof(int) + 256)) return rc;
-  if (int rc = g_hw.misc[7].reserve(numDmvr * 8 + 64)) return rc;
-  if (numPus) B200_CUDA(cudaMemcpyAsync(g_hw.misc[5].p, pus, numPus * sizeof(b200_pu), cudaMemcpyHostToDevice, s));
-  int* meta = g_hw.misc[6].as<int>(); uint32_t* tiles = reinterpret_cast<uint32_t*>(meta + LM_INTS);
-  if (int rc = launch_mc_bucket(g_hw.misc[5].as<b200_pu>(), numPus, tiles, capTiles, meta, *g, numSlots, wp ? numWp : 0, numDmvr, s)) return rc;
-  L.tiles = tiles; L.meta = meta;
-  if (wp && numWp > 0) {
-    if (int rc = g_hw.misc[2].reserve(numWp * sizeof(b200_wp))) return rc;
-    B200_CUDA(cudaMemcpyAsync(g_hw.misc[2].p, wp, numWp * sizeof(b200_wp), cudaMemcpyHostToDevice, s));
-    L.wp = g_hw.misc[2].as<b200_wp>();
-  }
-  if (int rc = fetch_list_meta(meta, L.cnt, MC_LISTS, "b200_mc_predict", s)) return rc;
-  B200_CUDA(cudaMemsetAsync(g_hw.misc[7].p, 0, numDmvr * 8 + 64, s));
-  memset(L.refs, 0, sizeof(L.refs)); for (size_t i = 0; i < ptrs.size(); i++) L.refs[i] = ptrs[i];
+  int* meta; uint32_t* tiles;
+  Staging st;
+  stage_picture(st, L.dst, dst, *g);
+  for (int sl = 0; sl < numSlots; sl++) stage_picture(st, &L.refs[sl * 3], &refs[sl * 3], *g);
+  st.add(&L.pus, pus, numPus); st.add(&meta, nullptr, LM_INTS); st.add(&tiles, nullptr, capTiles); st.add(&L.dmvrMv, nullptr, dmvrMv ? numDmvr * 2 : 0);
+  st.add(&L.wp, wp, wp && numWp > 0 ? numWp : 0);
+  if (int rc = st.commit(g_hw.buf, s)) return rc;
   for (int c = 0; c < 3; c++) L.refStride[c] = g->stride[c];
-  L.pus = g_hw.misc[5].as<b200_pu>(); L.dmvrMv = dmvrMv ? g_hw.misc[7].as<int32_t>() : nullptr;
+  if (int rc = launch_mc_bucket(L.pus, numPus, tiles, capTiles, meta, *g, numSlots, wp ? numWp : 0, numDmvr, s)) return rc;
+  L.tiles = tiles; L.meta = meta;
+  if (int rc = fetch_list_meta(meta, L.cnt, MC_LISTS, "b200_mc_predict", s)) return rc;
+  if (L.dmvrMv) B200_CUDA(cudaMemsetAsync(L.dmvrMv, 0, numDmvr * 8, s));
   StreamSet ss(s);
   if (int rc = launch_mc(L, ss)) return rc;
   if (int rc = download_planes(g, dst, L.dst, s)) return rc;
-  if (dmvrMv && numDmvr) B200_CUDA(cudaMemcpyAsync(dmvrMv, g_hw.misc[7].p, numDmvr * 8, cudaMemcpyDeviceToHost, s));
+  if (L.dmvrMv) B200_CUDA(cudaMemcpyAsync(dmvrMv, L.dmvrMv, numDmvr * 8, cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaStreamSynchronize(s));
   return 0;
 }

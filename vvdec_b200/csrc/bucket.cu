@@ -112,26 +112,26 @@ __global__ void __launch_bounds__(256) tu_scatter_kernel(const b200_tu* __restri
   if (ok) idx[base[c] + my] = (uint32_t)i;
 }
 
-int launch_mc_bucket(const b200_pu* pus, size_t numPus, uint32_t* tiles, size_t capTiles, int* meta, const b200_geom& g, int numSlots, int numWp, size_t numDmvr, cudaStream_t s)
+int launch_mc_bucket(const b200_pu* pus, size_t numPus, uint32_t* tiles, size_t capTiles, int* meta, const b200_geom& g, int numSlots, int numWp, size_t numDmvr, cudaStream_t s, KHook* hook)
 {
   const PuLimits lim = pu_limits(g, numSlots, numWp, numDmvr);
   B200_CUDA(cudaMemsetAsync(meta, 0, LM_INTS * sizeof(int), s));
   if (!numPus) return 0;
   const int grid = (int)((numPus + 255) / 256);
-  mc_count_kernel<<<grid, 256, 0, s>>>(pus, (int)numPus, meta, lim, (int)capTiles);
-  mc_scatter_kernel<<<grid, 256, 0, s>>>(pus, (int)numPus, meta, tiles, lim);
+  mc_count_kernel<<<grid, 256, 0, s>>>(pus, (int)numPus, meta, lim, (int)capTiles); hook_count(hook);
+  mc_scatter_kernel<<<grid, 256, 0, s>>>(pus, (int)numPus, meta, tiles, lim); hook_count(hook);
   B200_CUDA(cudaGetLastError());
   return 0;
 }
 
-int launch_tu_bucket(const b200_tu* tus, size_t numTus, uint32_t* idx, int* meta, const b200_geom& g, size_t numCoefs, size_t numScaling, cudaStream_t s)
+int launch_tu_bucket(const b200_tu* tus, size_t numTus, uint32_t* idx, int* meta, const b200_geom& g, size_t numCoefs, size_t numScaling, cudaStream_t s, KHook* hook)
 {
   const TuLimits lim = tu_limits(g, numCoefs, numScaling);
   B200_CUDA(cudaMemsetAsync(meta, 0, LM_INTS * sizeof(int), s));
   if (!numTus) return 0;
   const int grid = (int)((numTus + 255) / 256);
-  tu_count_kernel<<<grid, 256, 0, s>>>(tus, (int)numTus, meta, lim);
-  tu_scatter_kernel<<<grid, 256, 0, s>>>(tus, (int)numTus, meta, idx, lim);
+  tu_count_kernel<<<grid, 256, 0, s>>>(tus, (int)numTus, meta, lim); hook_count(hook);
+  tu_scatter_kernel<<<grid, 256, 0, s>>>(tus, (int)numTus, meta, idx, lim); hook_count(hook);
   B200_CUDA(cudaGetLastError());
   return 0;
 }
@@ -153,10 +153,10 @@ __global__ void __launch_bounds__(256) ctu_validate_kernel(const b200_sao_ctu* _
   if ((sao && sao_ctu_problem(sao[i], 3)) || (alf && alf_ctu_problem(alf[i], i, lim)) || (ctuSlice && ctuSlice[i] >= lim.numLfSlices)) atomicOr(&meta[LM_ERR], 4);
 }
 
-int launch_ctu_validate(const b200_sao_ctu* sao, const b200_alf_ctu* alf, const uint8_t* ctuSlice, int nCtu, const CtuLimits& lim, int* meta, cudaStream_t s)
+int launch_ctu_validate(const b200_sao_ctu* sao, const b200_alf_ctu* alf, const uint8_t* ctuSlice, int nCtu, const CtuLimits& lim, int* meta, cudaStream_t s, KHook* hook)
 {
   if (!nCtu || (!sao && !alf && !ctuSlice)) return 0;
-  ctu_validate_kernel<<<(nCtu + 255) / 256, 256, 0, s>>>(sao, alf, ctuSlice, nCtu, lim, meta);
+  ctu_validate_kernel<<<(nCtu + 255) / 256, 256, 0, s>>>(sao, alf, ctuSlice, nCtu, lim, meta); hook_count(hook);
   B200_CUDA(cudaGetLastError());
   return 0;
 }

@@ -84,19 +84,19 @@ template <int C> __global__ void __launch_bounds__(256) fg_kernel(const FgParams
 
 // tables: device copies (pattern 64 KB, sLUT / pLUT 768 B each, lineSeeds); seeds: scratch of nbx * nby words
 int launch_film_grain(const DevPlanes& src, const DevPlanes& dst, const b200_geom& g, const int8_t* pattern, const uint8_t* sLUT, const uint8_t* pLUT,
-                      const uint32_t* lineSeeds, uint32_t* seeds, int scaleShift, const uint8_t present[3], cudaStream_t s)
+                      const uint32_t* lineSeeds, uint32_t* seeds, int scaleShift, const uint8_t present[3], cudaStream_t s, KHook* hook)
 {
   FgParams P;
   for (int c = 0; c < 3; c++) { P.src[c] = src.p[c]; P.dst[c] = dst.p[c]; P.srcStride[c] = src.stride[c]; P.dstStride[c] = dst.stride[c]; P.present[c] = present[c]; }
   P.W = g.width; P.H = g.height; P.bs = g.bitDepth - 8; P.scaleShift = scaleShift; P.nbx = (g.width + 15) / 16;
   P.pattern = pattern; P.sLUT = sLUT; P.pLUT = pLUT; P.seeds = seeds;
   const int nby = (g.height + 15) / 16;
-  fg_seed_kernel<<<(nby + 63) / 64, 64, 0, s>>>(lineSeeds, P.nbx, nby, seeds);
-  fg_kernel<0><<<dim3((g.width + 63) / 64, (g.height + 3) / 4), 256, 0, s>>>(P);
+  fg_seed_kernel<<<(nby + 63) / 64, 64, 0, s>>>(lineSeeds, P.nbx, nby, seeds); hook_count(hook);
+  fg_kernel<0><<<dim3((g.width + 63) / 64, (g.height + 3) / 4), 256, 0, s>>>(P); hook_count(hook);
   if (g.chromaFormat) {
     const dim3 grd((g.width / 2 + 63) / 64, (g.height / 2 + 3) / 4);
-    fg_kernel<1><<<grd, 256, 0, s>>>(P);
-    fg_kernel<2><<<grd, 256, 0, s>>>(P);
+    fg_kernel<1><<<grd, 256, 0, s>>>(P); hook_count(hook);
+    fg_kernel<2><<<grd, 256, 0, s>>>(P); hook_count(hook);
   }
   B200_CUDA(cudaGetLastError());
   return 0;

@@ -104,7 +104,7 @@ __global__ void hash_finish_kernel(const uint32_t* acc, int method, int nPl, uin
 }
 
 // acc: 3 zero-initialised words (device), digest: 12 bytes (device)
-int launch_hash(const DevPlanes& src, const b200_geom& g, int method, uint32_t* acc, uint8_t* digest, cudaStream_t s)
+int launch_hash(const DevPlanes& src, const b200_geom& g, int method, uint32_t* acc, uint8_t* digest, cudaStream_t s, KHook* hook)
 {
   const int nPl = g.chromaFormat ? 3 : 1, two = g.bitDepth > 8;
   uint32_t initMul[2] = {1, 1};
@@ -117,14 +117,14 @@ int launch_hash(const DevPlanes& src, const b200_geom& g, int method, uint32_t* 
       P.warpMul = crc_xpow(bitsPerSample * HASH_WARP);
       if (c < 2) initMul[c] = crc_xpow(bitsPerSample * (unsigned long long)P.N);
       const long long threads = (P.N + P.pad) / HASH_CHUNK;
-      crc_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(P);
+      crc_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(P); hook_count(hook);
     } else {
       for (int k = 0; k < 5; k++) P.c[k] = 0; P.warpMul = 0;
       dim3 grd((P.W + 127) / 128, (P.H + 7) / 8);
-      checksum_kernel<<<grd, 256, 0, s>>>(P);
+      checksum_kernel<<<grd, 256, 0, s>>>(P); hook_count(hook);
     }
   }
-  hash_finish_kernel<<<1, 32, 0, s>>>(acc, method, nPl, initMul[0], initMul[1], digest);
+  hash_finish_kernel<<<1, 32, 0, s>>>(acc, method, nPl, initMul[0], initMul[1], digest); hook_count(hook);
   B200_CUDA(cudaGetLastError());
   return 0;
 }

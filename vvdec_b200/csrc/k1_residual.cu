@@ -285,10 +285,10 @@ k1_residual_kernel(const b200_tu* __restrict__ tus, const uint32_t* __restrict__
   k1_tu<CLS>(tus, (int)idx[meta[LM_OFF + CLS] + i], coefs, scaling, p0, p1, p2, r0, r1, r2, s0, s1, s2, bitDepth, mode, compSel, vpduScale, vpduGeo, s_c[grp], s_t[grp], lane);
 }
 
-int launch_k1_residual(const K1Launch& L, StreamSet& ss, KProf* prof)
+int launch_k1_residual(const K1Launch& L, StreamSet& ss, KHook* hook)
 {
   if (L.numTus == 0) return 0;
-  if (prof) prof->begin(B200_KF_K1, ss.main);
+  hook_begin(hook, B200_KF_K1, ss.main);
   const int vs = L.geom.ctuSize == 128 ? 64 : L.geom.ctuSize;
   int vpduGeo = 0; while ((1 << (vpduGeo + 1)) <= vs) vpduGeo++;
   vpduGeo |= ((L.geom.width + vs - 1) / vs) << 8;
@@ -301,14 +301,13 @@ int launch_k1_residual(const K1Launch& L, StreamSet& ss, KProf* prof)
 #define K1_GO(C) k1_residual_kernel<C><<<grid, K1Cfg<C>::THREADS, 0, s>>>(L.tus, L.idx, L.meta, L.coefs, L.scaling, L.planes.p[0], L.planes.p[1], L.planes.p[2], L.resi[0], L.resi[1], L.resi[2], \
                                                                    L.planes.stride[0], L.planes.stride[1], L.planes.stride[2], L.geom.bitDepth, L.mode, L.compSel, L.vpduScale, vpduGeo)
     switch (c) { case 0: K1_GO(0); break; case 1: K1_GO(1); break; case 2: K1_GO(2); break; default: K1_GO(3); break; }
+    hook_count(hook);
 #undef K1_GO
     B200_CUDA(cudaGetLastError());
   }
   ss.join();
-  if (prof) prof->end(B200_KF_K1, ss.main);
+  hook_end(hook, B200_KF_K1, ss.main);
   return 0;
 }
-
-int k1_launch_count(const K1Launch& L) { int n = 0; for (int c = 0; c < K1_LISTS; c++) n += L.cnt[c] > 0; return n; }
 
 }  // namespace b200

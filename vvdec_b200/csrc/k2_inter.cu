@@ -919,7 +919,7 @@ __global__ void __launch_bounds__(256) mc_affine_kernel(const McParams P)
 static void (*const kMcKernels[4][2])(const McParams, int) = {
   {mc_kernel<0, 1>, mc_kernel<0, 4>}, {mc_kernel<1, 1>, mc_kernel<1, 4>}, {nullptr, mc_kernel<2, 4>}, {nullptr, mc_kernel<3, 4>}};
 
-int launch_mc(const McLaunch& L, StreamSet& ss, KProf* prof)
+int launch_mc(const McLaunch& L, StreamSet& ss, KHook* hook)
 {
   McParams P;
   for (int c = 0; c < 3; c++) { P.dst[c] = L.dst.p[c]; P.dstStride[c] = L.dst.stride[c]; P.refStride[c] = L.refStride[c]; }
@@ -930,20 +930,19 @@ int launch_mc(const McLaunch& L, StreamSet& ss, KProf* prof)
   P.wp = L.wp;
   P.lmcs = L.lmcs; P.lmcsLog2 = 0; { int o = (1 << L.geom.bitDepth) / 16; while ((1 << (P.lmcsLog2 + 1)) <= o) P.lmcsLog2++; }
   int launched = 0;
-  if (prof) prof->begin(B200_KF_MC_TILE, ss.main);
+  hook_begin(hook, B200_KF_MC_TILE, ss.main);
   for (int m = 3; m >= 0; m--) for (int k = 3; k >= 0; k--) {      // heaviest lists first (DMVR 16x16 ... uni 8x4)
     const int nsamp = 32 << k, list = m * 4 + k, grid = L.cnt[list];
     if (!grid || (m >= 2 && k < 2)) continue;
     cudaStream_t s = ss.pick(launched++);
     kMcKernels[m][k >= 2]<<<grid, k >= 2 ? nsamp >> 2 : nsamp, (size_t)mc_smem_elems(m, k) * 2, s>>>(P, list);
+    hook_count(hook);
     B200_CUDA(cudaGetLastError());
   }
-  if (L.cnt[16]) { cudaStream_t s = ss.pick(launched++); mc_affine_kernel<<<L.cnt[16], 256, 0, s>>>(P); B200_CUDA(cudaGetLastError()); }
+  if (L.cnt[16]) { cudaStream_t s = ss.pick(launched++); mc_affine_kernel<<<L.cnt[16], 256, 0, s>>>(P); hook_count(hook); B200_CUDA(cudaGetLastError()); }
   ss.join();
-  if (prof) prof->end(B200_KF_MC_TILE, ss.main);      // with forked streams the affine tiles are inside the same interval
+  hook_end(hook, B200_KF_MC_TILE, ss.main);      // with forked streams the affine tiles are inside the same interval
   return 0;
 }
-
-int mc_launch_count(const McLaunch& L) { int n = L.cnt[16] > 0; for (int m = 0; m < 4; m++) for (int k = 0; k < 4; k++) n += L.cnt[m * 4 + k] > 0 && !(m >= 2 && k < 2); return n; }
 
 }  // namespace b200

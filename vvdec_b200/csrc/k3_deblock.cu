@@ -258,7 +258,7 @@ __global__ void __launch_bounds__(256, 3) lf_kernel(const LfParams P, const LfSl
   }
 }
 
-int launch_lf_deblock(const LfLaunch& L, cudaStream_t s, KProf* prof)
+int launch_lf_deblock(const LfLaunch& L, cudaStream_t s, KHook* hook)
 {
   LfParams P;
   for (int c = 0; c < 3; c++) { P.plane[c] = L.planes.p[c]; P.stride[c] = L.planes.stride[c]; }
@@ -267,8 +267,8 @@ int launch_lf_deblock(const LfLaunch& L, cudaStream_t s, KProf* prof)
   P.ctusW = (P.W + P.ctuSize - 1) >> P.ctuLog2; P.chroma = L.geom.chromaFormat == 1;
   P.ctuSlice = L.ctuSlice; P.seq = L.seq;
   dim3 blk(32, 8), grd((P.W4 + 31) / 32, (P.H4 + 7) / 8);
-  if (L.dirs & 1) { if (prof) prof->begin(B200_KF_LF_V, s); P.grid = L.lfV; lf_kernel<0><<<grd, blk, 0, s>>>(P, L.slices); B200_CUDA(cudaGetLastError()); if (prof) prof->end(B200_KF_LF_V, s); }
-  if (L.dirs & 2) { if (prof) prof->begin(B200_KF_LF_H, s); P.grid = L.lfH; lf_kernel<1><<<grd, blk, 0, s>>>(P, L.slices); B200_CUDA(cudaGetLastError()); if (prof) prof->end(B200_KF_LF_H, s); }
+  if (L.dirs & 1) { hook_begin(hook, B200_KF_LF_V, s); P.grid = L.lfV; lf_kernel<0><<<grd, blk, 0, s>>>(P, L.slices); hook_count(hook); B200_CUDA(cudaGetLastError()); hook_end(hook, B200_KF_LF_V, s); }
+  if (L.dirs & 2) { hook_begin(hook, B200_KF_LF_H, s); P.grid = L.lfH; lf_kernel<1><<<grd, blk, 0, s>>>(P, L.slices); hook_count(hook); B200_CUDA(cudaGetLastError()); hook_end(hook, B200_KF_LF_H, s); }
   return 0;
 }
 

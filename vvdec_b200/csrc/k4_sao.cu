@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(256) sao_kernel(const SaoParams P)
   *dptr = o;
 }
 
-int launch_sao(const SaoLaunch& L, cudaStream_t s, KProf* prof)
+int launch_sao(const SaoLaunch& L, cudaStream_t s, KHook* hook)
 {
   SaoParams P;
   for (int c = 0; c < 3; c++) { P.src[c] = L.src.p[c]; P.dst[c] = L.dst.p[c]; P.stride[c] = L.src.stride[c]; }
@@ -124,10 +124,10 @@ int launch_sao(const SaoLaunch& L, cudaStream_t s, KProf* prof)
   P.ctusW = (P.W + P.ctuSize - 1) / P.ctuSize; P.chroma = L.geom.chromaFormat == 1;
   P.ctus = L.ctus; P.vb = L.vb;
   dim3 blk(32, 8), grd((P.W / 4 + 31) / 32, (P.H + 7) / 8, P.chroma ? 3 : 1);
-  if (prof) prof->begin(B200_KF_SAO, s);
-  sao_kernel<<<grd, blk, 0, s>>>(P);
+  hook_begin(hook, B200_KF_SAO, s);
+  sao_kernel<<<grd, blk, 0, s>>>(P); hook_count(hook);
   B200_CUDA(cudaGetLastError());
-  if (prof) prof->end(B200_KF_SAO, s);
+  hook_end(hook, B200_KF_SAO, s);
   return 0;
 }
 

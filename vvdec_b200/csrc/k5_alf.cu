@@ -384,7 +384,7 @@ __global__ void __launch_bounds__(256) alf_chroma_kernel(const AlfParams P)
   *reinterpret_cast<uint2*>(P.dst[c] + (size_t)y * stride + x) = o;
 }
 
-int launch_alf(const AlfLaunch& L, StreamSet& ss, KProf* prof)
+int launch_alf(const AlfLaunch& L, StreamSet& ss, KHook* hook)
 {
   cudaStream_t s = ss.main;
   AlfParams P;
@@ -399,15 +399,15 @@ int launch_alf(const AlfLaunch& L, StreamSet& ss, KProf* prof)
   if (L.geom.chromaFormat == 1) {                           // chroma + CC-ALF only read the SAO output: runs beside the luma kernel
     cudaStream_t sc = ss.pick(0);
     dim3 blk(32, 8), grd(((P.W >> 1) / 4 + 31) / 32, ((P.H >> 1) + 7) / 8, 2);
-    if (prof) prof->begin(B200_KF_ALF_CHROMA, sc);
-    alf_chroma_kernel<<<grd, blk, 0, sc>>>(P);
+    hook_begin(hook, B200_KF_ALF_CHROMA, sc);
+    alf_chroma_kernel<<<grd, blk, 0, sc>>>(P); hook_count(hook);
     B200_CUDA(cudaGetLastError());
-    if (prof) prof->end(B200_KF_ALF_CHROMA, sc);
+    hook_end(hook, B200_KF_ALF_CHROMA, sc);
   }
-  if (prof) prof->begin(B200_KF_ALF_LUMA, s);
-  alf_luma_kernel<<<grdL, 256, 0, s>>>(P);
+  hook_begin(hook, B200_KF_ALF_LUMA, s);
+  alf_luma_kernel<<<grdL, 256, 0, s>>>(P); hook_count(hook);
   B200_CUDA(cudaGetLastError());
-  if (prof) prof->end(B200_KF_ALF_LUMA, s);
+  hook_end(hook, B200_KF_ALF_LUMA, s);
   ss.join();
   return 0;
 }

@@ -675,19 +675,19 @@ __global__ void __launch_bounds__(128) intra_ciip_clear_kernel(const b200_intra_
   }
 }
 
-int launch_intra_ciip_clear(const b200_intra_tu* tus, size_t numTus, int16_t* const resi[3], const int stride[3], cudaStream_t s)
+int launch_intra_ciip_clear(const b200_intra_tu* tus, size_t numTus, int16_t* const resi[3], const int stride[3], cudaStream_t s, KHook* hook)
 {
   if (!numTus) return 0;
   const int grid = (int)std::min<size_t>(numTus, (size_t)2 * num_sms());
-  intra_ciip_clear_kernel<<<grid, 128, 0, s>>>(tus, (int)numTus, resi[0], resi[1], resi[2], stride[0], stride[1], stride[2]);
+  intra_ciip_clear_kernel<<<grid, 128, 0, s>>>(tus, (int)numTus, resi[0], resi[1], resi[2], stride[0], stride[1], stride[2]); hook_count(hook);
   B200_CUDA(cudaGetLastError());
   return 0;
 }
 
-int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_geom& g, int* meta, cudaStream_t s)
+int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_geom& g, int* meta, cudaStream_t s, KHook* hook)
 {
   if (!numTus) return 0;
-  intra_validate_kernel<<<(unsigned)((numTus + 255) / 256), 256, 0, s>>>(tus, (int)numTus, g, meta);
+  intra_validate_kernel<<<(unsigned)((numTus + 255) / 256), 256, 0, s>>>(tus, (int)numTus, g, meta); hook_count(hook);
   B200_CUDA(cudaGetLastError());
   return 0;
 }
@@ -696,9 +696,10 @@ int launch_intra_validate(const b200_intra_tu* tus, size_t numTus, const b200_ge
 // (bench.py --lanes 1, I_picture_ms): 1x 10.15 ms, 1.5x 9.64, 2x 9.56, 3x 9.43, SM count (132 CTAs) 9.42 — 3x is the smallest factor that costs nothing
 constexpr int kWaveCtasPerDiag2 = 6;
 
-int launch_intra(const IntraLaunch& L, cudaStream_t s)
+int launch_intra(const IntraLaunch& L, cudaStream_t s, KHook* hook)
 {
   if (!L.numTus) return 0;
+  hook_begin(hook, B200_KF_INTRA, s);
   IntraParams P;
   for (int c = 0; c < 3; c++) { P.planes[c] = L.planes.p[c]; P.resi[c] = L.resi[c]; P.stride[c] = L.planes.stride[c]; P.owner[c] = L.owner[c]; P.ownerStride[c] = L.ownerStride[c]; }
   if (!L.geom.chromaFormat) { P.planes[1] = P.planes[2] = nullptr; }
@@ -721,7 +722,7 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
   const bool dense = L.numTus >= 48 * std::max<size_t>(1, (size_t)L.geom.width * L.geom.height >> 14);                   // >= 48 blocks per 128x128 luma area
   const bool v1 = !L.order || force1 || (!force2 && !dense) || ((P.stride[0] | P.stride[1] | P.stride[2]) & 1);          // the tile loads move 32-bit words
   const unsigned grid = (unsigned)((L.numTus + 255) / 256);
-  if (!cont) intra_owner_kernel<<<(unsigned)L.numTus, 64, 0, s>>>(P);
+  if (!cont) { intra_owner_kernel<<<(unsigned)L.numTus, 64, 0, s>>>(P); hook_count(hook); }
   if (!v1) {
     // v2: per-CTU runs of the list (decoding order keeps a CTU's blocks together), CTUs in wave-front order, one CTA per CTU at a time
     const size_t nCtu = (size_t)P.ctusW * P.ctusH;
@@ -730,9 +731,9 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
     else {
       B200_CUDA(cudaMemsetAsync(P.ctuCnt, 0, nCtu * sizeof(int), s));
       B200_CUDA(cudaMemsetAsync(P.ctuFirst, 0x7f, nCtu * sizeof(int), s));
-      intra_ctu_count_kernel<<<grid, 256, 0, s>>>(P);
-      intra_ctu_check_kernel<<<grid, 256, 0, s>>>(P);
-      intra_ctu_order_kernel<<<1, 1024, nCtu * sizeof(int), s>>>(P, ctuOrder, counters);
+      intra_ctu_count_kernel<<<grid, 256, 0, s>>>(P); hook_count(hook);
+      intra_ctu_check_kernel<<<grid, 256, 0, s>>>(P); hook_count(hook);
+      intra_ctu_order_kernel<<<1, 1024, nCtu * sizeof(int), s>>>(P, ctuOrder, counters); hook_count(hook);
     }
     // Grid: as many CTAs as the wave front can keep busy.  Only the CTUs of about one key x + 2 y (at most `diag` of them) run at a time — with the next
     // key's CTUs trailing them by a fraction of a CTU — and each CTA fills an SM (registers and shared memory), so a grid of SM count would hold SMs that
@@ -749,8 +750,9 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
     // 128x5 9.56 ms, 128x6 9.99 ms
     static bool attr = false;
     if (!attr) { B200_CUDA(cudaFuncSetAttribute(intra_ctu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)V2_SMEM)); attr = true; }
-    intra_ctu_kernel<<<ctas, V2_THREADS, V2_SMEM, s>>>(P, ctuOrder, counters);
+    intra_ctu_kernel<<<ctas, V2_THREADS, V2_SMEM, s>>>(P, ctuOrder, counters); hook_count(hook);
     B200_CUDA(cudaGetLastError());
+    hook_end(hook, B200_KF_INTRA, s);
     return 0;
   }
   const char* order = getenv("B200_INTRA_ORDER");                // measurement and test switch, read on every launch: "decode" = tickets in list order
@@ -761,15 +763,16 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s)
     if (!cont) {
       B200_CUDA(cudaMemsetAsync(P.ctuCnt, 0, nCtu * sizeof(int), s));
       B200_CUDA(cudaMemsetAsync(P.ctuFirst, 0x7f, nCtu * sizeof(int), s));
-      intra_ctu_count_kernel<<<grid, 256, 0, s>>>(P);
-      intra_ctu_base_kernel<<<1, 1, 0, s>>>(P);
-      intra_perm_kernel<<<grid, 256, 0, s>>>(P, perm);
+      intra_ctu_count_kernel<<<grid, 256, 0, s>>>(P); hook_count(hook);
+      intra_ctu_base_kernel<<<1, 1, 0, s>>>(P); hook_count(hook);
+      intra_perm_kernel<<<grid, 256, 0, s>>>(P, perm); hook_count(hook);
     }
     P.perm = perm;
   }
   const int ctas = (int)std::min<size_t>(L.numTus, (size_t)num_sms() * 12);
-  intra_kernel<<<ctas, IT_THREADS, 0, s>>>(P);
+  intra_kernel<<<ctas, IT_THREADS, 0, s>>>(P); hook_count(hook);
   B200_CUDA(cudaGetLastError());
+  hook_end(hook, B200_KF_INTRA, s);
   return 0;
 }
 

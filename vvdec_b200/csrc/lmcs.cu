@@ -62,29 +62,33 @@ __global__ void __launch_bounds__(256) lmcs_validate_kernel(const b200_lmcs_vpdu
   if (i < numVpdus && lmcs_vpdu_problem(vpdus[i], i, g)) atomicOr(&meta[LM_ERR], 16);
 }
 
-int launch_lmcs_validate(const b200_lmcs_vpdu* vpdus, const b200_geom& g, int* meta, cudaStream_t s)
+int launch_lmcs_validate(const b200_lmcs_vpdu* vpdus, const b200_geom& g, int* meta, cudaStream_t s, KHook* hook)
 {
   const int vs = g.ctuSize == 128 ? 64 : g.ctuSize;
   const int n = ((g.width + vs - 1) / vs) * ((g.height + vs - 1) / vs);
-  lmcs_validate_kernel<<<(n + 255) / 256, 256, 0, s>>>(vpdus, n, g, meta);
+  lmcs_validate_kernel<<<(n + 255) / 256, 256, 0, s>>>(vpdus, n, g, meta); hook_count(hook);
   B200_CUDA(cudaGetLastError());
   return 0;
 }
 
-int launch_lmcs_vpdu(const LmcsLaunch& L, cudaStream_t s)
+int launch_lmcs_vpdu(const LmcsLaunch& L, cudaStream_t s, KHook* hook)
 {
   const int vs = L.geom.ctuSize == 128 ? 64 : L.geom.ctuSize;
   const int n = ((L.geom.width + vs - 1) / vs) * ((L.geom.height + vs - 1) / vs);
-  lmcs_vpdu_kernel<<<(n + 7) / 8, 256, 0, s>>>(L.planes.p[0], L.planes.stride[0], L.geom.width, L.geom.height, L.geom.bitDepth, vs, L.lmcs, L.vpdus, n, L.scale);
+  hook_begin(hook, B200_KF_LMCS, s);
+  lmcs_vpdu_kernel<<<(n + 7) / 8, 256, 0, s>>>(L.planes.p[0], L.planes.stride[0], L.geom.width, L.geom.height, L.geom.bitDepth, vs, L.lmcs, L.vpdus, n, L.scale); hook_count(hook);
   B200_CUDA(cudaGetLastError());
+  hook_end(hook, B200_KF_LMCS, s);
   return 0;
 }
 
-int launch_lmcs_inv(const LmcsLaunch& L, cudaStream_t s)
+int launch_lmcs_inv(const LmcsLaunch& L, cudaStream_t s, KHook* hook)
 {
   dim3 grd((L.geom.width + 255) / 256, (L.geom.height + 7) / 8);
-  lmcs_inv_kernel<<<grd, 256, sizeof(int16_t) << L.geom.bitDepth, s>>>(L.planes.p[0], L.planes.stride[0], L.geom.width, L.geom.height, L.geom.bitDepth, L.invLut);
+  hook_begin(hook, B200_KF_LMCS, s);
+  lmcs_inv_kernel<<<grd, 256, sizeof(int16_t) << L.geom.bitDepth, s>>>(L.planes.p[0], L.planes.stride[0], L.geom.width, L.geom.height, L.geom.bitDepth, L.invLut); hook_count(hook);
   B200_CUDA(cudaGetLastError());
+  hook_end(hook, B200_KF_LMCS, s);
   return 0;
 }
 

@@ -35,12 +35,12 @@ __global__ void __launch_bounds__(256) narrow8_kernel(const int16_t* __restrict_
   for (int k = 0; k < 4; k++) if (x + k < W) o[k] = (uint8_t)(p[k] >> shift);
 }
 
-int launch_pack(const DevPlanes& src, const b200_geom& g, int fmt, uint8_t* const dst[3], cudaStream_t s)
+int launch_pack(const DevPlanes& src, const b200_geom& g, int fmt, uint8_t* const dst[3], cudaStream_t s, KHook* hook)
 {
   for (int c = 0; c < (g.chromaFormat ? 3 : 1); c++) {
     const int W = c ? g.width >> 1 : g.width, H = c ? g.height >> 1 : g.height;
-    if (fmt == B200_OUT_PYUV) { dim3 grd((W + 255) / 256, (H + 7) / 8); pack_pyuv_kernel<<<grd, 256, 0, s>>>(src.p[c], src.stride[c], W, H, dst[c]); }
-    else                      { dim3 grd((W + 127) / 128, (H + 7) / 8); narrow8_kernel<<<grd, 256, 0, s>>>(src.p[c], src.stride[c], W, H, g.bitDepth - 8, dst[c]); }
+    if (fmt == B200_OUT_PYUV) { dim3 grd((W + 255) / 256, (H + 7) / 8); pack_pyuv_kernel<<<grd, 256, 0, s>>>(src.p[c], src.stride[c], W, H, dst[c]); hook_count(hook); }
+    else                      { dim3 grd((W + 127) / 128, (H + 7) / 8); narrow8_kernel<<<grd, 256, 0, s>>>(src.p[c], src.stride[c], W, H, g.bitDepth - 8, dst[c]); hook_count(hook); }
   }
   B200_CUDA(cudaGetLastError());
   return 0;
