@@ -13,6 +13,9 @@ static int ilog2(int v) { int r = 0; while (v > 1) { v >>= 1; r++; } return r; }
 static int iclip(int lo, int hi, int v) { return v < lo ? lo : v > hi ? hi : v; }
 static int imin(int a, int b) { return a < b ? a : b; }
 static int imax(int a, int b) { return a > b ? a : b; }
+/* the probe of one record (orc_intra_probe): the unclipped range [lo, hi] at a clip site; NULL on the normal path */
+static void seen(int32_t* lo, int32_t* hi, int v) { if (v < *lo) *lo = v; if (v > *hi) *hi = v; }
+#define PROBE(site, v) do { if (pr) seen(&pr->site##Min, &pr->site##Max, (v)); } while (0)
 
 static const int kAng[32] = {0, 1, 2, 3, 4, 6, 8, 10, 12, 14, 16, 18, 20, 23, 26, 29, 32, 35, 39, 45, 51, 57, 64, 73, 86, 102, 128, 171, 256, 341, 512, 1024};
 static const int kInvAng[32] = {0, 16384, 8192, 5461, 4096, 2731, 2048, 1638, 1365, 1170, 1024, 910, 819, 712, 630, 565,
@@ -32,7 +35,7 @@ static int wide_angle(int w, int h, int mode)     /* getWideAngle :443 */
 
 /* ref: (2h + mrl + 1) rows x stride (= 2w + 1 + mrl); row 0 = top-left + above row, column 0 = left column (reference layout) */
 static void fill_ref(const int16_t* plane, ptrdiff_t ps, int x0, int y0, int w, int h, int mrl, int unitW, int unitH, int availTL, int numAbove, int numLeft,
-                     int bitDepth, int16_t* ref, int stride)
+                     int bitDepth, int16_t* ref, int stride, orc_intra_trace* pr)
 {
   const int predSize = 2 * w, predHSize = 2 * h;
   const int totalUnits = (predSize + unitW - 1) / unitW + (predHSize + unitH - 1) / unitH + 1;
@@ -41,6 +44,7 @@ static void fill_ref(const int16_t* plane, ptrdiff_t ps, int x0, int y0, int w, 
   if (n == 0) {
     for (int j = 0; j <= predSize + mrl; j++) ref[j] = (int16_t)dc;
     for (int i = 1; i <= predHSize + mrl; i++) ref[i * stride] = (int16_t)dc;
+    PROBE(subst, dc);
   } else if (n == totalUnits) {
     const int16_t* p = src - (1 + mrl) * ps - (1 + mrl);
     for (int j = 0; j <= predSize + mrl; j++) ref[j] = p[j];
@@ -51,7 +55,7 @@ static void fill_ref(const int16_t* plane, ptrdiff_t ps, int x0, int y0, int w, 
     int16_t* d = ref + (1 + mrl) * stride;
     int t = imin(numLeft * unitH, predHSize);
     for (int i = 0; i < t; i++) d[i * stride] = p[i * ps];
-    for (int i = t; i < predHSize; i++) d[i * stride] = d[(t - 1) * stride];
+    for (int i = t; i < predHSize; i++) { d[i * stride] = d[(t - 1) * stride]; PROBE(subst, d[i * stride]); }
     if (availTL) {
       p = src - (1 + mrl) * ps - (1 + mrl);
       for (int j = 0; j <= mrl; j++) ref[j] = p[j];
@@ -60,25 +64,27 @@ static void fill_ref(const int16_t* plane, ptrdiff_t ps, int x0, int y0, int w, 
       const int16_t v = src[-(1 + mrl)];
       ref[0] = v;
       for (int i = 1; i <= mrl; i++) { ref[i] = v; ref[i * stride] = v; }
+      PROBE(subst, v);
     }
     d = ref + 1 + mrl;
     if (numAbove) {
       p = src - ps * (1 + mrl);
       t = imin(numAbove * unitW, predSize);
       for (int j = 0; j < t; j++) d[j] = p[j];
-      for (int j = t; j < predSize; j++) d[j] = d[t - 1];
-    } else for (int j = 0; j < predSize; j++) d[j] = d[-1];
+      for (int j = t; j < predSize; j++) { d[j] = d[t - 1]; PROBE(subst, d[j]); }
+    } else for (int j = 0; j < predSize; j++) { d[j] = d[-1]; PROBE(subst, d[j]); }
   } else {
     const int16_t* p = src - ps * (1 + mrl);
     int16_t* d = ref + 1 + mrl;
     const int t = imin(numAbove * unitW, predSize);
     for (int j = 0; j < t; j++) d[j] = p[j];
-    for (int j = t; j < predSize; j++) d[j] = d[t - 1];
+    for (int j = t; j < predSize; j++) { d[j] = d[t - 1]; PROBE(subst, d[j]); }
     const int16_t v = p[0];
     ref[0] = v;
     for (int i = 1; i <= mrl; i++) { ref[i] = v; ref[i * stride] = v; }
     d = ref + (1 + mrl) * stride;
     for (int i = 0; i < predHSize; i++) d[i * stride] = v;
+    PROBE(subst, v);
   }
 }
 
@@ -115,7 +121,7 @@ static void pred_planar(const int16_t* src, int stride, int w, int h, int16_t* d
 /* topLen / leftLen: m_topRefLength / m_leftRefLength (2w / 2h for a regular block; CU size + partition size with ISP); waW x waH: the size the wide-angle
  * mapping looks at (the CU with ISP); isp: always the cubic filter (:745) */
 static void pred_angular_ex(const int16_t* src, int stride, int w0, int h0, int chroma, int dirMode, int mrl, int doPDPC, int pmax, int16_t* dst, ptrdiff_t ds,
-                            int topLen, int leftLen, int waW, int waH, int isp)
+                            int topLen, int leftLen, int waW, int waH, int isp, orc_intra_trace* pr)
 {
   int w = w0, h = h0;
   const int predMode = wide_angle(waW, waH, dirMode), ver = predMode >= 34;
@@ -148,7 +154,11 @@ static void pred_angular_ex(const int16_t* src, int stride, int w0, int h0, int 
       const int topLeft = AT(0, 0);
       for (int y = 0; y < h; y++) {
         const int left = refSide[y + 1];
-        for (int x = 0; x < lev[scale]; x++) { const int wL = 32 >> imin(31, (x << 1) >> scale); out[y * ts + x] = (int16_t)iclip(0, pmax, (wL * (left - topLeft) + refMain[x + 1] * 64 + 32) >> 6); }
+        for (int x = 0; x < lev[scale]; x++) {
+          const int wL = 32 >> imin(31, (x << 1) >> scale), v = (wL * (left - topLeft) + refMain[x + 1] * 64 + 32) >> 6;
+          PROBE(pdpc, v);
+          out[y * ts + x] = (int16_t)iclip(0, pmax, v);
+        }
         for (int x = lev[scale]; x < w; x++) out[y * ts + x] = refMain[x + 1];
       }
     } else for (int y = 0; y < h; y++) for (int x = 0; x < w; x++) out[y * ts + x] = refMain[x + 1];
@@ -159,6 +169,7 @@ static void pred_angular_ex(const int16_t* src, int stride, int w0, int h0, int 
         const int diff = imin(abs(predMode - 18), abs(predMode - 50)), log2Size = (ilog2(w) + ilog2(h)) >> 1;
         const int interpolationFlag = diff > kIntraFilterThr[0][log2Size];       /* filterFlag, and the angle is fractional here */
         const int cubic = isp || !interpolationFlag || mrl > 0;
+        if (pr) pr->interp = cubic ? 1 : 2;
         for (int y = 0; y < h; y++, deltaPos += angle) {
           const int dI = deltaPos >> 5, dF = deltaPos & 31;
           int f[4];
@@ -167,11 +178,12 @@ static void pred_angular_ex(const int16_t* src, int stride, int w0, int h0, int 
           for (int x = 0; x < w; x++) {
             const int16_t* p = refMain + dI + x;
             int v = (int16_t)((f[0] * p[0] + f[1] * p[1] + f[2] * p[2] + f[3] * p[3] + 32) >> 6);
-            if (cubic) v = iclip(0, pmax, v);
+            if (cubic) { PROBE(cubic, v); v = iclip(0, pmax, v); }
             out[y * ts + x] = (int16_t)v;
           }
         }
       } else {
+        if (pr) pr->interp = 3;
         for (int y = 0; y < h; y++, deltaPos += angle) {
           const int dI = deltaPos >> 5, dF = deltaPos & 31;
           for (int x = 0; x < w; x++) out[y * ts + x] = (int16_t)(((32 - dF) * refMain[dI + 1 + x] + dF * refMain[dI + 2 + x] + 16) >> 5);
@@ -202,7 +214,7 @@ static void pred_angular_ex(const int16_t* src, int stride, int w0, int h0, int 
  * first entry), computeReducedPred :281-330 (matrix stage, transposed variant), predictionUpsampling :233-262 / predictionUpsampling1D :190-230
  * (linear interpolation, horizontally on the rows of the reduced prediction, then vertically), initPredBlockParams :139-160; size classes
  * getMipSizeId (UnitTools.cpp:3748); weights MipData.h (shift 6, offset 32). */
-static void pred_mip(const int16_t* src, int stride, int w, int h, int modeIdx, int transpose, int bitDepth, int16_t* dst, ptrdiff_t ds)
+static void pred_mip(const int16_t* src, int stride, int w, int h, int modeIdx, int transpose, int bitDepth, int16_t* dst, ptrdiff_t ds, orc_intra_trace* pr)
 {
   const int sizeId = (w == 4 && h == 4) ? 0 : (w == 4 || h == 4 || (w == 8 && h == 8)) ? 1 : 2;
   const int bdry = sizeId == 0 ? 2 : 4, red = sizeId < 2 ? 4 : 8, upH = w / red, upV = h / red, inSize = 2 * bdry;
@@ -220,6 +232,7 @@ static void pred_mip(const int16_t* src, int stride, int w, int h, int modeIdx, 
   int* input = transpose ? inT : in;
   const int inputOffset = input[0];
   input[0] = sizeId < 2 ? (1 << (bitDepth - 1)) - inputOffset : 0;
+  if (pr) { pr->mipSizeId = sizeId; pr->mipInputOffset = inputOffset; pr->mipInput0 = input[0]; }
   for (int i = 1; i < inSize; i++) input[i] -= inputOffset;
   const uint8_t* weight = sizeId == 0 ? &kMip4x4[modeIdx * 64] : sizeId == 1 ? &kMip8x8[modeIdx * 128] : &kMip16x16[modeIdx * 448];
   const int redSize = sizeId == 2;
@@ -230,6 +243,7 @@ static void pred_mip(const int16_t* src, int stride, int w, int h, int modeIdx, 
     int acc = offset;
     for (int i = redSize; i < inSize; i++) acc += input[i] * weight[i - redSize];
     weight += inSize - redSize;
+    PROBE(mip, (acc >> 6) + inputOffset);
     const int v = iclip(0, pmax, (acc >> 6) + inputOffset);
     if (transpose) R[(pos % red) * red + pos / red] = v; else R[pos] = v;
   }
@@ -246,7 +260,8 @@ static void pred_mip(const int16_t* src, int stride, int w, int h, int modeIdx, 
         const int before = j == 0 ? left[(kk + 1) * upV - 1] : R[kk * red + j - 1], behind = R[kk * red + j];
         hv[q] = (int16_t)((int16_t)(before * upH + (upH >> 1)) + (ii + 1) * (int16_t)(behind - before)) >> l2H;
       }
-      dst[y * ds + x] = upV == 1 ? (int16_t)hv[1] : (int16_t)(((int16_t)(hv[0] * upV + (upV >> 1)) + (i + 1) * (int16_t)(hv[1] - hv[0])) >> l2V);
+      /* the reference accumulates in Pel and shifts the wrapped sum (predictionUpsampling1D :219-224): at 12 bit x 16 the sum leaves int16 */
+      dst[y * ds + x] = upV == 1 ? (int16_t)hv[1] : (int16_t)((int16_t)((int16_t)(hv[0] * upV + (upV >> 1)) + (i + 1) * (int16_t)(hv[1] - hv[0])) >> l2V);
     }
 }
 
@@ -346,10 +361,11 @@ static void pred_cclm(const b200_geom* g, const int16_t* luma, ptrdiff_t ls, con
   for (int j = 0; j < h; j++) for (int i = 0; i < w; i++) dst[j * ds + i] = (int16_t)iclip(0, pmax, ((p.a * d0[j * CCLM_TS + i]) >> p.shift) + p.b);
 }
 
-static void pred_angular(const int16_t* src, int stride, int w0, int h0, int chroma, int dirMode, int mrl, int filtered, int doPDPC, int pmax, int16_t* dst, ptrdiff_t ds)
+static void pred_angular(const int16_t* src, int stride, int w0, int h0, int chroma, int dirMode, int mrl, int filtered, int doPDPC, int pmax, int16_t* dst, ptrdiff_t ds,
+                         orc_intra_trace* pr)
 {
   (void)filtered;
-  pred_angular_ex(src, stride, w0, h0, chroma, dirMode, mrl, doPDPC, pmax, dst, ds, 2 * w0, 2 * h0, w0, h0, 0);
+  pred_angular_ex(src, stride, w0, h0, chroma, dirMode, mrl, doPDPC, pmax, dst, ds, 2 * w0, 2 * h0, w0, h0, 0, pr);
 }
 
 /* Intra sub-partitions (ISP), luma of one CU.  Follows IntraPrediction::initIntraPatternChTypeISP :966-1070 (the CU's reference samples are fetched
@@ -364,7 +380,7 @@ void orc_intra_isp_cu(const b200_geom* g, int16_t* luma, const int16_t* resi, in
   const ptrdiff_t ps = g->stride[0];
   const int pmax = (1 << g->bitDepth) - 1, S = 2 * w + 1, rows = 2 * h + 1;
   int16_t* B = (int16_t*)calloc((size_t)S * rows + 64, sizeof(int16_t));
-  fill_ref(luma, ps, x0, y0, w, h, 0, 4, 4, availTL, numAbove, numLeft, g->bitDepth, B, S);
+  fill_ref(luma, ps, x0, y0, w, h, 0, 4, 4, availTL, numAbove, numLeft, g->bitDepth, B, S, NULL);
   const int hor = ispMode == 1, split = hor ? h : w, nonSplit = hor ? w : h;
   const int part = imax(split >> 2, nonSplit < 16 ? 16 / nonSplit : 1), nParts = split / part;
   const int regDiff = !hor && (w == 4 || (w == 8 && h > 4));                       /* vertical split with partitions narrower than 4: predict 4 wide */
@@ -396,7 +412,7 @@ void orc_intra_isp_cu(const b200_geom* g, int16_t* luma, const int16_t* resi, in
         if (rw <= rh) for (int i = 0; i < rh; i++) sum += AT(0, 1 + i);
         const int16_t dc = (int16_t)((sum + (denom >> 1)) >> ilog2(denom));
         for (int y = 0; y < rh; y++) for (int x = 0; x < rw; x++) dst[y * ps + x] = dc;
-      } else pred_angular_ex(src, stride, rw, rh, 0, dirMode, 0, doPDPC, pmax, dst, ps, topLen, leftLen, w, h, 1);
+      } else pred_angular_ex(src, stride, rw, rh, 0, dirMode, 0, doPDPC, pmax, dst, ps, topLen, leftLen, w, h, 1, NULL);
       if (doPDPC && dirMode <= 1) {
         const int scale = (ilog2(rw) - 2 + ilog2(rh) - 2 + 2) >> 2;
         for (int y = 0; y < rh; y++) {
@@ -429,7 +445,7 @@ static void intra_isp_region(const b200_geom* g, int16_t* luma, const b200_intra
   const int pmax = (1 << g->bitDepth) - 1, S = 2 * w + 1, rows = 2 * h + 1, dirMode = t->mode;
   const int leftAvail = t->lmLeft, aboveAvail = t->lmAbove;
   int16_t* B = (int16_t*)calloc((size_t)S * rows + 64, sizeof(int16_t));
-  fill_ref(luma, ps, x0, y0, w, h, 0, 4, 4, (t->flags & B200_INTRA_AVAIL_TL) ? 1 : 0, t->numAbove, t->numLeft, g->bitDepth, B, S);
+  fill_ref(luma, ps, x0, y0, w, h, 0, 4, 4, (t->flags & B200_INTRA_AVAIL_TL) ? 1 : 0, t->numAbove, t->numLeft, g->bitDepth, B, S, NULL);
   int16_t* W = B + oy * S + ox;
   const int topLen = w + rw, leftLen = h + rh;
   const int16_t* rec = luma + (ptrdiff_t)(y0 + oy) * ps + x0 + ox;
@@ -454,7 +470,7 @@ static void intra_isp_region(const b200_geom* g, int16_t* luma, const b200_intra
     if (rw <= rh) for (int i = 0; i < rh; i++) sum += AT(0, 1 + i);
     const int16_t dc = (int16_t)((sum + (denom >> 1)) >> ilog2(denom));
     for (int y = 0; y < rh; y++) for (int x = 0; x < rw; x++) dst[y * ps + x] = dc;
-  } else pred_angular_ex(src, stride, rw, rh, 0, dirMode, 0, doPDPC, pmax, dst, ps, topLen, leftLen, w, h, 1);
+  } else pred_angular_ex(src, stride, rw, rh, 0, dirMode, 0, doPDPC, pmax, dst, ps, topLen, leftLen, w, h, 1, NULL);
   if (doPDPC && dirMode <= 1) {
     const int scale = (ilog2(rw) - 2 + ilog2(rh) - 2 + 2) >> 2;
     for (int y = 0; y < rh; y++) {
@@ -479,21 +495,21 @@ void orc_cclm_params(const b200_geom* g, int16_t* const planes[3], const b200_in
   const int w = 1 << t->log2w, h = 1 << t->log2h, stride = 2 * w + 1, rows = 2 * h + 1;
   int16_t* ref = (int16_t*)calloc((size_t)stride * rows + 64, sizeof(int16_t));
   static _Thread_local int16_t tmp[(64 + 1) * CCLM_TS + CCLM_TS];
-  fill_ref(planes[t->comp], g->stride[t->comp], t->x, t->y, w, h, 0, 2, 2, (t->flags & B200_INTRA_AVAIL_TL) ? 1 : 0, t->numAbove, t->numLeft, g->bitDepth, ref, stride);
+  fill_ref(planes[t->comp], g->stride[t->comp], t->x, t->y, w, h, 0, 2, 2, (t->flags & B200_INTRA_AVAIL_TL) ? 1 : 0, t->numAbove, t->numLeft, g->bitDepth, ref, stride, NULL);
   cclm_derive(g, planes[0], g->stride[0], ref, stride, t, tmp + CCLM_TS + 1, out);
   free(ref);
 }
 
-void orc_intra_tu(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* t)
+static void intra_tu(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* t, orc_intra_trace* pr)
 {
   if (t->flags & B200_INTRA_ISP) { intra_isp_region(g, planes[0], t); return; }
   const int c = t->comp, w = 1 << t->log2w, h = 1 << t->log2h, mrl = c ? 0 : t->multiRefIdx, pmax = (1 << g->bitDepth) - 1;
   const int unit = c ? 2 : 4, stride = 2 * w + 1 + mrl, rows = 2 * h + 1 + mrl;
   int16_t* ref = (int16_t*)calloc((size_t)stride * rows * 2 + 64, sizeof(int16_t));
   int16_t* flt = ref + (size_t)stride * rows + 32;
-  fill_ref(planes[c], g->stride[c], t->x, t->y, w, h, mrl, unit, unit, (t->flags & B200_INTRA_AVAIL_TL) ? 1 : 0, t->numAbove, t->numLeft, g->bitDepth, ref, stride);
+  fill_ref(planes[c], g->stride[c], t->x, t->y, w, h, mrl, unit, unit, (t->flags & B200_INTRA_AVAIL_TL) ? 1 : 0, t->numAbove, t->numLeft, g->bitDepth, ref, stride, pr);
   const int16_t* src = ref;
-  if ((t->flags & B200_INTRA_FILTER_REF) && !c && !mrl) { filter_ref(ref, flt, w, h); src = flt; }
+  if ((t->flags & B200_INTRA_FILTER_REF) && !c && !mrl) { filter_ref(ref, flt, w, h); src = flt; if (pr) pr->filtered = 1; }
   int16_t* dst = planes[c] + (ptrdiff_t)t->y * g->stride[c] + t->x;
   const ptrdiff_t ds = g->stride[c];
   int16_t* inter = NULL;                                        /* CIIP: the block holds the inter prediction; keep it for the blend */
@@ -510,8 +526,8 @@ void orc_intra_tu(const b200_geom* g, int16_t* const planes[3], const b200_intra
   } else if (t->mode == B200_INTRA_BDPCM_HOR) { for (int y = 0; y < h; y++) for (int x = 0; x < w; x++) dst[y * ds + x] = AT(0, y + 1); }
   else if (t->mode == B200_INTRA_BDPCM_VER) { for (int y = 0; y < h; y++) for (int x = 0; x < w; x++) dst[y * ds + x] = AT(x + 1, 0); }
   else if (t->mode >= B200_INTRA_LM) pred_cclm(g, planes[0], g->stride[0], src, stride, t, dst, ds);
-  else if (t->mode == B200_INTRA_MIP) pred_mip(src, stride, w, h, t->mip & 0x7f, t->mip >> 7, g->bitDepth, dst, ds);
-  else pred_angular(src, stride, w, h, c != 0, t->mode, mrl, 0, doPDPC, pmax, dst, ds);
+  else if (t->mode == B200_INTRA_MIP) pred_mip(src, stride, w, h, t->mip & 0x7f, t->mip >> 7, g->bitDepth, dst, ds, pr);
+  else pred_angular(src, stride, w, h, c != 0, t->mode, mrl, 0, doPDPC, pmax, dst, ds, pr);
   if (doPDPC && t->mode <= B200_INTRA_DC) {                    /* IntraPredSampleFilterCore :212 */
     const int scale = (t->log2w - 2 + t->log2h - 2 + 2) >> 2;
     for (int y = 0; y < h; y++) {
@@ -527,8 +543,11 @@ void orc_intra_tu(const b200_geom* g, int16_t* const planes[3], const b200_intra
     for (int y = 0; y < h; y++) for (int x = 0; x < w; x++) dst[y * ds + x] = (int16_t)((wM * inter[y * w + x] + wI * dst[y * ds + x] + 2) >> 2);
     free(inter);
   }
+  if (pr) for (int y = 0; y < h; y++) for (int x = 0; x < w; x++) PROBE(pred, dst[y * ds + x]);
   free(ref);
 }
+
+void orc_intra_tu(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* t) { intra_tu(g, planes, t, NULL); }
 
 void orc_intra_predict(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* tus, size_t numTus)
 {
@@ -536,20 +555,33 @@ void orc_intra_predict(const b200_geom* g, int16_t* const planes[3], const b200_
 }
 
 /* prediction + reconstruction (DecCu.cpp:390-398): blocks flagged B200_INTRA_ADD_RESI become clip(pred + resi) before the next block reads them */
-void orc_intra_reconstruct(const b200_geom* g, int16_t* const planes[3], const int16_t* const resi[3], const b200_intra_tu* tus, size_t numTus)
+static void reconstruct_tu(const b200_geom* g, int16_t* const planes[3], const int16_t* const resi[3], const b200_intra_tu* t, orc_intra_trace* pr)
 {
   const int pmax = (1 << g->bitDepth) - 1;
-  for (size_t i = 0; i < numTus; i++) {
-    const b200_intra_tu* t = &tus[i];
-    orc_intra_tu(g, planes, t);
-    if (resi && resi[t->comp] && (t->flags & B200_INTRA_ADD_RESI)) {
-      const int isp = t->flags & B200_INTRA_ISP, tw = isp ? orc_isp_tu_width(t) : 1 << t->log2w;
-      for (int y = 0; y < (1 << t->log2h); y++)
-        for (int x = 0; x < (1 << t->log2w); x++) {
-          if (isp && !((t->ciip >> (x / tw)) & 1)) continue;                 /* transform units of the region without a residual */
-          const ptrdiff_t o = (ptrdiff_t)(t->y + y) * g->stride[t->comp] + t->x + x;
-          planes[t->comp][o] = (int16_t)iclip(0, pmax, planes[t->comp][o] + resi[t->comp][o]);
-        }
-    }
+  intra_tu(g, planes, t, pr);
+  if (resi && resi[t->comp] && (t->flags & B200_INTRA_ADD_RESI)) {
+    const int isp = t->flags & B200_INTRA_ISP, tw = isp ? orc_isp_tu_width(t) : 1 << t->log2w;
+    for (int y = 0; y < (1 << t->log2h); y++)
+      for (int x = 0; x < (1 << t->log2w); x++) {
+        if (isp && !((t->ciip >> (x / tw)) & 1)) continue;                 /* transform units of the region without a residual */
+        const ptrdiff_t o = (ptrdiff_t)(t->y + y) * g->stride[t->comp] + t->x + x;
+        PROBE(reco, planes[t->comp][o] + resi[t->comp][o]);
+        planes[t->comp][o] = (int16_t)iclip(0, pmax, planes[t->comp][o] + resi[t->comp][o]);
+      }
   }
+}
+
+void orc_intra_reconstruct(const b200_geom* g, int16_t* const planes[3], const int16_t* const resi[3], const b200_intra_tu* tus, size_t numTus)
+{
+  for (size_t i = 0; i < numTus; i++) reconstruct_tu(g, planes, resi, &tus[i], NULL);
+}
+
+/* one record as orc_intra_reconstruct runs it (the planes advance), and what its prediction went through */
+void orc_intra_probe(const b200_geom* g, int16_t* const planes[3], const int16_t* const resi[3], const b200_intra_tu* t, orc_intra_trace* out)
+{
+  memset(out, 0, sizeof(*out));
+  out->substMin = out->cubicMin = out->pdpcMin = out->mipMin = out->recoMin = out->predMin = INT32_MAX;
+  out->substMax = out->cubicMax = out->pdpcMax = out->mipMax = out->recoMax = out->predMax = INT32_MIN;
+  out->mipSizeId = -1;
+  reconstruct_tu(g, planes, resi, t, out);
 }

@@ -77,6 +77,18 @@ void orc_intra_reconstruct(const b200_geom* g, int16_t* const planes[3], const i
  * template; normDiff (-1 without a slope) and whether shift < 1 clamped the slope; blkMin / blkMax: the range of the block's down-sampled luma.  Reads the planes as orc_intra_tu would at that point of a list. */
 typedef struct orc_cclm { int32_t a, b, shift, minL, maxL, minC, maxC, cntT, cntL, normDiff, clamped, selL[4], selC[4], blkMin, blkMax; } orc_cclm;
 void orc_cclm_params(const b200_geom* g, int16_t* const planes[3], const b200_intra_tu* t, orc_cclm* out);
+/* What the prediction of one regular intra record went through.  Each xxxMin / xxxMax pair is the range of the values a clip site saw before it clipped
+ * (INT32_MAX / INT32_MIN where the record never reached it): cubic: the 4-tap cubic interpolation of a fractional luma angle; pdpc: PDPC of the
+ * horizontal / vertical modes; mip: the reduced MIP prediction; reco: pred + resi; pred: the final prediction (before the residual).  subst: the
+ * values reference substitution wrote (1 << (bitDepth - 1) without any neighbour, else the padding copied from available samples).  filtered: the
+ * [1 2 1] filtered reference was used; interp: 0 none, 1 cubic, 2 Gaussian (luma), 3 two-tap linear (chroma); mipSizeId (-1: not MIP),
+ * mipInputOffset (the first down-sampled boundary sample) and mipInput0 (the first matrix input after the rebase). */
+typedef struct orc_intra_trace {
+  int32_t substMin, substMax, cubicMin, cubicMax, pdpcMin, pdpcMax, mipMin, mipMax, recoMin, recoMax, predMin, predMax;
+  int32_t filtered, interp, mipSizeId, mipInputOffset, mipInput0;
+} orc_intra_trace;
+/* one record as orc_intra_reconstruct runs it (prediction, then pred + resi where the record adds a residual and resi is not NULL): the planes advance */
+void orc_intra_probe(const b200_geom* g, int16_t* const planes[3], const int16_t* const resi[3], const b200_intra_tu* t, orc_intra_trace* out);
 /* film grain synthesis, per-sample part (FilmGrainImpl::add_grain_block); tables as FilmGrainImpl holds them after FilmGrain::updateFGC:
  * pattern [2][8][64][64], sLUT / pLUT [3][256], lineSeeds [(h+15)/16] (FilmGrain::prepareBlockSeeds); 4:2:0, planes in place */
 void orc_film_grain(int16_t* const planes[3], const ptrdiff_t strides[3], int w, int h, int bitDepth, const int8_t* pattern, const uint8_t* sLUT,

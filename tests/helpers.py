@@ -26,6 +26,24 @@ def cclm_params(oracle, g, planes, rec):
     return out
 
 
+class IntraProbe(C.Structure):
+    """orc_intra_trace (oracle/vvc_oracle.h): what the oracle's prediction of one regular intra record went through."""
+    _fields_ = [(n, C.c_int32) for n in ("substMin", "substMax", "cubicMin", "cubicMax", "pdpcMin", "pdpcMax", "mipMin", "mipMax", "recoMin", "recoMax",
+                                         "predMin", "predMax", "filtered", "interp", "mipSizeId", "mipInputOffset", "mipInput0")]
+
+
+def intra_probes(oracle, g, planes, recs, resi=None):
+    """orc_intra_probe of every record of a list, run in list order over copies of `planes` (as orc_intra_reconstruct runs it with `resi`)."""
+    work = [None if p is None else p.copy() for p in planes]
+    out = []
+    for r in recs:
+        one = np.array(r, abi.INTRA_TU_DTYPE).reshape(1)
+        pr = IntraProbe()
+        oracle.orc_intra_probe(C.byref(g), abi.plane_ptrs(work), None if resi is None else abi.plane_ptrs(resi), one.ctypes.data, C.byref(pr))
+        out.append(pr)
+    return out
+
+
 def load_oracle():
     srcs = [os.path.join(ROOT, "oracle", f) for f in os.listdir(os.path.join(ROOT, "oracle")) if f.endswith((".c", ".h"))]
     if not os.path.exists(ORACLE_SO) or any(os.path.getmtime(s) > os.path.getmtime(ORACLE_SO) for s in srcs):
@@ -67,6 +85,7 @@ def load_oracle():
     lib.orc_intra_isp_cu.argtypes = [C.POINTER(abi.Geom), i16p, C.c_void_p] + [C.c_int] * 11 + [C.c_uint]
     lib.orc_intra_reconstruct.argtypes = [C.POINTER(abi.Geom), PL, PL, C.c_void_p, C.c_size_t]
     lib.orc_cclm_params.argtypes = [C.POINTER(abi.Geom), PL, C.c_void_p, C.POINTER(Cclm)]
+    lib.orc_intra_probe.argtypes = [C.POINTER(abi.Geom), PL, PL, C.c_void_p, C.POINTER(IntraProbe)]
     lib.orc_film_grain.argtypes = [PL, C.POINTER(C.c_ssize_t), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.orc_plane_hash.argtypes = [C.c_int, C.c_int, i16p, C.c_ssize_t, C.c_int, C.c_int, u8p]
     return lib

@@ -12,9 +12,9 @@ pytestmark = pytest.mark.ref
 CHROMA_MODES = [0, 1, 18, 50, 2, 34, 66, 70, 70, 70, 23, 45, 61]       # 70 = DM (PU::getFinalIntraMode -> the luma mode)
 
 
-def run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, k, dirL, dirC, mrl, bdpcm, bdpcmC=0, mip=0, colloc=0, paint=None, out=None):
+def run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, k, dirL, dirC, mrl, bdpcm, bdpcmC=0, mip=0, colloc=0, paint=None, out=None, resi=None):
     """paint(planes): writes designed neighbour samples into the noise planes before the reference runs; out: a list the reference's planes are
-    appended to."""
+    appended to; resi: residual planes the predicted CU adds (clip(pred + resi)), else prediction only."""
     g = abi.make_geom(W, H, bd, ctu=ctu)
     planes = synth.noise_planes(rng, W, H, bd)
     if paint: paint(planes)
@@ -27,19 +27,22 @@ def run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, k, dirL, dirC, mrl, 
     luma_only = w < 8 or (w // 2) * (h // 2) < 16                       # such luma blocks are CUs of a local dual tree: no chroma of their own
     cus[k]["rsv"][0] = luma_only
     cus[k]["rsv"][2] = mip                                           # bit 0 MIP (dirL = MIP mode index), bit 1 transposed
+    cus[k]["rsv"][1] = resi is not None                              # add the residual
     want = [p.copy() for p in planes]
     recs = np.zeros(3, abi.INTRA_TU_DTYPE)
-    n = ref.ref_intra_case(simd, C.byref(g), abi.plane_ptrs(want), None, cus.ctypes.data, k + 1, 0, recs.ctypes.data, 3, colloc)
+    n = ref.ref_intra_case(simd, C.byref(g), abi.plane_ptrs(want), None if resi is None else abi.plane_ptrs(resi), cus.ctypes.data, k + 1, 0, recs.ctypes.data, 3, colloc)
     assert n == (1 if luma_only else 3), n
     recs = recs[:n]
     got = [p.copy() for p in planes]
-    oracle.orc_intra_predict(C.byref(g), abi.plane_ptrs(got), recs.ctypes.data, n)
+    if resi is None: oracle.orc_intra_predict(C.byref(g), abi.plane_ptrs(got), recs.ctypes.data, n)
+    else: oracle.orc_intra_reconstruct(C.byref(g), abi.plane_ptrs(got), abi.plane_ptrs(resi), recs.ctypes.data, n)
     for c in range(3):
         assert np.array_equal(got[c], want[c]), (c, layout[k], dirL, dirC, mrl, bdpcm, recs[c])
     assert not np.array_equal(want[0][y:y + h, x:x + w], planes[0][y:y + h, x:x + w])
     # the synthetic generator used by the GPU tests derives the same records (availability from the decoding order, filter decision, DM)
     mine = synth.gen_intra_records(rng, layout, W, H, modes={k: (dirL, dirC, mrl, bdpcm, mip)}, upto=k, colloc=colloc)
     mine = mine[-n:]
+    if resi is not None: mine["flags"] |= abi.INTRA_ADD_RESI
     for f in ("x", "y", "log2w", "log2h", "comp", "mode", "multiRefIdx", "flags", "numAbove", "numLeft", "mip", "lmAbove", "lmLeft"):
         assert np.array_equal(mine[f], recs[f]), (f, mine[f], recs[f], layout[k])
     if out is not None: out.append(want)
@@ -158,6 +161,72 @@ def test_intra_cclm_designed(oracle, ref, bd, simd, colloc):
         assert got == t, (dirC, t, got, sl)
         reached.add((dirC, t))
     assert len(reached) == len(jobs)
+
+
+def _designed_jobs(bd):
+    """(w, h, dirL, mrl, bdpcm, mip, pattern, value, where, residual) of the designed regular-intra blocks run through the reference: the blocks of
+    synth.intra_designed_sweep's targets and flat cases, at the position the layout gives them.  Every target x shape class is kept: cubic modes with
+    MRL 0 / 1 / 2 and PDPC of modes 18 / 50 on every luma shape (chroma: the same modes as DM), BDPCM H / V, every MIP mode of one shape per size class
+    (plain and transposed, both patterns; 4x64 and 64x4 up-sample by 16), no neighbour at the picture corner and padding from the left column at the top edge; flat references on
+    every shape with a sample of modes.  Residuals of +-3/4 pmax on the pdpc, BDPCM and substitution blocks."""
+    out = []
+    pmax, mid = (1 << bd) - 1, 1 << (bd - 1)
+    for i, (w, h) in enumerate(synth.INTRA_LUMA_SHAPES):
+        for mrl in (0, 1, 2):
+            if mrl and h == 64: continue                             # the interior position is not on the first row of a CTU, but keep the CTU case's rule
+            out += [(w, h, m, mrl, 0, 0, "cubic", 0, "inner", False) for m in synth.intra_cubic_modes(w, h, mrl)[:2]]
+        out += [(w, h, m, 0, 0, 0, "pdpc", 0, "inner", True) for m in (18, 50)]
+        if w <= 32 and h <= 32: out += [(w, h, 0, 0, b, 0, "bdpcm", 0, "inner", True) for b in (1, 2)]
+        out += [(w, h, (1, 66, 2)[i % 3], 0, 0, 0, None, 0, "corner", True), (w, h, (0, 50, 18)[i % 3], 0, 0, 0, "pad", (0, pmax)[i & 1], "top", True)]
+        fm = [0, 1, 2, 18, 34, 50, 66] + [3 + (7 * i + 5 * j) % 63 for j in range(4)]
+        out += [(w, h, m, (j % 3) * (m > 1 and h < 64), 0, 0, "flat", (0, 1, mid, pmax - 1, pmax)[(i + j) % 5], "inner", False) for j, m in enumerate(fm)]
+    for (w, h) in ((4, 4), (8, 8), (16, 16), (4, 64), (64, 4)):       # 4x64 / 64x4: up-sampling by 16, which wraps the reference's int16 sums at 12 bit
+        out += [(w, h, m, 0, 0, 1 | (tr << 1), p, 0, "inner", False) for m in range(synth.intra_mip_modes(w, h)) for tr in (0, 1) for p in ("mip_a", "mip_b")]
+    return out
+
+
+@pytest.mark.parametrize("bd,simd", [(8, 0), (8, 1), (10, 0), (10, 1), (12, 0)])
+def test_intra_designed_vs_ref(oracle, ref, bd, simd):
+    """Regular intra prediction on the designed references of synth.intra_designed_sweep (the targets and flat cases), painted around the predicted
+    CU, the reference's planes against the oracle's (prediction, or pred + resi where a residual is given).  Every clip site reaches below 0 and above
+    pmax, substitution takes the mid value and pads 0 / pmax, as the oracle's probe says.  The 12-bit case runs the C kernels only (see
+    test_intra_random_layouts)."""
+    from tests.helpers import intra_probes
+    rng = np.random.default_rng(bd * 2 + simd)
+    W, H, ctu = 256, 128, 128
+    pmax = (1 << bd) - 1
+    layouts = {"inner": ([(0, 0, 64, 64), (64, 0, 64, 64), (0, 64, 64, 64)], (64, 64)), "corner": ([], (0, 0)), "top": ([(0, 0, 64, 64)], (64, 0))}
+    reached = set()
+    for (w, h, dirL, mrl, bdpcm, mip, pattern, v, where, add) in _designed_jobs(bd):
+        before, (x, y) = layouts[where]
+        layout = before + [(x, y, w, h)]
+
+        def paint(planes):
+            if pattern is None: return
+            pat = synth._intra_pattern(pattern, bd, v)
+            synth._intra_paint(planes[0], x, y, w, h, 4, pat)
+            for c in (1, 2): synth._intra_paint(planes[c], x // 2, y // 2, max(w // 2, 2), max(h // 2, 2), 2, pat)
+        resi = [rng.integers(-(3 * pmax) // 4, (3 * pmax) // 4 + 1, size=(H >> (c > 0), W >> (c > 0))).astype(np.int16) for c in range(3)] if add else None
+        want = []
+        recs = run_case(oracle, ref, rng, W, H, bd, ctu, simd, layout, len(before), dirL, 70, mrl, bdpcm, mip=mip, paint=paint, out=want, resi=resi)
+        before_planes = [p.copy() for p in want[0]]                  # the probe re-runs the records over the reference's output, where the neighbours are unchanged
+        g = abi.make_geom(W, H, bd, ctu=ctu)
+        for r, p in zip(recs, intra_probes(oracle, g, before_planes, recs, resi)):
+            c = int(r["comp"]) > 0
+            if p.cubicMin < 0: reached.add(("cubic_lo", mrl))
+            if p.cubicMax > pmax: reached.add(("cubic_hi", mrl))
+            if p.pdpcMin < 0: reached.add(("pdpc_lo", c))
+            if p.pdpcMax > pmax: reached.add(("pdpc_hi", c))
+            if p.mipSizeId >= 0 and p.mipMin < 0: reached.add(("mip_lo", p.mipSizeId))
+            if p.mipSizeId >= 0 and p.mipMax > pmax: reached.add(("mip_hi", p.mipSizeId))
+            if (p.substMin, p.substMax) == (1 << (bd - 1),) * 2 and r["numAbove"] + r["numLeft"] == 0: reached.add(("subst_mid", c))
+            if pattern == "pad" and (p.substMin, p.substMax) == (v, v): reached.add(("pad", v, c))
+            if resi is not None and p.recoMin < 0: reached.add(("reco_lo", c))
+            if resi is not None and p.recoMax > pmax: reached.add(("reco_hi", c))
+            if pattern == "flat": assert (p.predMin, p.predMax) == (v, v), (r, v)
+    want = {(t, m) for t in ("cubic_lo", "cubic_hi") for m in (0, 1, 2)} | {(t, c) for t in ("pdpc_lo", "pdpc_hi", "subst_mid", "reco_lo", "reco_hi") for c in (False, True)}
+    want |= {(t, s) for t in ("mip_lo", "mip_hi") for s in range(3)} | {("pad", v, c) for v in (0, pmax) for c in (False, True)}
+    assert want <= reached, sorted(want - reached)
 
 
 @pytest.mark.parametrize("w,h", [(8, 8), (16, 16), (32, 32), (64, 64), (16, 8), (8, 16), (64, 16), (16, 64), (32, 8), (4, 16), (16, 4)])

@@ -1,7 +1,8 @@
 """The K6 test lists reach what tests/test_k6_intra_gpu.py claims they reach (no device needed): the designed sweep holds every block it lists and no
 block of it reads another, and the generated cases put more than 1024 records into one CTU, stay below the density threshold where they stand for a B
 picture, and never use MRL on the first row of a CTU.  The designed CCLM sweep reaches every geometry and parameter-derivation target it claims (as the
-oracle derives them), and the rules refuse each malformed CCLM record on the host."""
+oracle derives them), and the rules refuse each malformed CCLM record on the host.  The designed sweep of regular modes (synth.intra_designed_sweep)
+reaches every clip and substitution target it claims, as the oracle's own prediction reports them (orc_intra_probe)."""
 import ctypes as C
 import numpy as np
 import pytest
@@ -115,7 +116,7 @@ def _cclm_reached(p, bd):
 
 def _rules_accept(case):
     g, recs = case["g"], case["recs"]
-    planes = [p.copy() for p in case["planes"]]
+    planes = [None if p is None else p.copy() for p in case["planes"]]
     rc = vvdec_b200.lib().b200_intra_reconstruct(C.byref(g), abi.plane_ptrs(planes), abi.plane_ptrs(case["resi"]), recs.ctypes.data, len(recs))
     assert rc in (0, -3), vvdec_b200.lib().b200_last_error()               # -3: no device (the host checks every record first)
 
@@ -230,3 +231,137 @@ def test_cclm_refusals_on_the_host(row):
     assert what.encode() in lib.b200_last_error(), (name, lib.b200_last_error())
     assert all(np.array_equal(a, b) for a, b in zip(got, planes))
     assert lib.b200_intra_reconstruct(C.byref(g), abi.plane_ptrs(got), abi.plane_ptrs(resi), ok.ctypes.data, len(ok)) in (0, -3)
+
+
+# ---- the designed sweep of regular modes (synth.intra_designed_sweep): what each case reaches, as the oracle's prediction reports it (orc_intra_probe)
+def _intra_reached(case, oracle):
+    """{(target, class)} the records of a case reach: the clip sites below 0 / above pmax per shape class, substitution values, pred + resi per
+    component, BDPCM predictions at 0 and pmax."""
+    pmax, mid = (1 << case["bd"]) - 1, 1 << (case["bd"] - 1)
+    got = set()
+    for r, tag, p in zip(case["recs"], case["tags"], helpers.intra_probes(oracle, case["g"], case["planes"], case["recs"], case["resi"])):
+        c, w, h, mrl = int(r["comp"]), 1 << int(r["log2w"]), 1 << int(r["log2h"]), int(r["multiRefIdx"])
+        if p.interp == 1 and p.cubicMin < 0: got.add(("cubic_lo", (w, h, mrl)))
+        if p.interp == 1 and p.cubicMax > pmax: got.add(("cubic_hi", (w, h, mrl)))
+        if p.pdpcMin < 0: got.add(("pdpc_lo", (c > 0, w, h, int(r["mode"]))))
+        if p.pdpcMax > pmax: got.add(("pdpc_hi", (c > 0, w, h, int(r["mode"]))))
+        if p.mipSizeId >= 0 and p.mipMin < 0: got.add(("mip_lo", (p.mipSizeId, int(r["mip"]) >> 7)))
+        if p.mipSizeId >= 0 and p.mipMax > pmax: got.add(("mip_hi", (p.mipSizeId, int(r["mip"]) >> 7)))
+        if p.mipSizeId >= 0: assert p.mipInput0 == ((1 << (case["bd"] - 1)) - p.mipInputOffset if p.mipSizeId < 2 else 0)
+        edge = "top" if r["y"] == 0 else "left" if r["x"] == 0 else "inner"
+        if (p.substMin, p.substMax) == (mid, mid) and r["numAbove"] + r["numLeft"] == 0: got.add(("subst_mid", (c > 0, edge)))
+        if (p.substMin, p.substMax) == (0, 0) and tag[0] == "pad": got.add(("pad_0", (c > 0, edge)))
+        if (p.substMin, p.substMax) == (pmax, pmax) and tag[0] == "pad": got.add(("pad_max", (c > 0, edge)))
+        if p.recoMin < 0: got.add(("reco_lo", c))
+        if p.recoMax > pmax: got.add(("reco_hi", c))
+        if r["mode"] in (abi.INTRA_BDPCM_HOR, abi.INTRA_BDPCM_VER) and (p.predMin, p.predMax) == (0, pmax): got.add(("bdpcm", (int(r["mode"]), w, h)))
+    return got
+
+
+@pytest.mark.parametrize("name", [n for n, v in synth.INTRA_SWEEP_CASES.items() if v[0] == "targets"])
+def test_intra_targets_reached(oracle, name):
+    """Every target of INTRA_TARGETS in every shape class the case holds: the cubic interpolation below 0 and above pmax for every luma shape with
+    MRL 0 (where the shape has a fractional cubic mode), 1 and 2; PDPC of modes 18 and 50 below 0 and above pmax on every luma and chroma shape; the
+    reduced MIP prediction below 0 and above pmax in every size class, transposed and not; the mid value without neighbours, and padding at 0 and pmax
+    from one unit, inside the picture and at its top and left edges; pred + resi below 0 and above pmax in every component; BDPCM H / V at 0 and pmax."""
+    case = synth.intra_designed_sweep(name)
+    ctu, chroma = case["ctu"], case["planes"][1] is not None
+    got = _intra_reached(case, oracle)
+    luma = [(w, h) for (w, h) in synth.INTRA_LUMA_SHAPES if w <= ctu and h <= ctu]
+    shapes = [(False, w, h) for (w, h) in luma] + ([(True, w, h) for (w, h) in synth.INTRA_CHROMA_SHAPES if w <= ctu // 2 and h <= ctu // 2] if chroma else [])
+    want = {(t, (w, h, mrl)) for t in ("cubic_lo", "cubic_hi") for (w, h) in luma for mrl in (0, 1, 2)
+            if synth.intra_cubic_modes(w, h, mrl) and not (mrl and h == ctu)}
+    want |= {(t, (c, w, h, m)) for t in ("pdpc_lo", "pdpc_hi") for (c, w, h) in shapes for m in (18, 50)}
+    want |= {(t, (s, tr)) for t in ("mip_lo", "mip_hi") for s in range(3) for tr in (0, 1)}
+    want |= {(t, (c, e)) for t in ("subst_mid", "pad_0", "pad_max") for c in ({False, True} if chroma else {False}) for e in ("inner", "top", "left")}
+    want -= {("pad_0", (c, "top")) for c in (False, True)} | {("pad_max", (c, "left")) for c in (False, True)}   # the edge blocks pad from pmax at the top, 0 at the left
+    want |= {(t, c) for t in ("reco_lo", "reco_hi") for c in (range(3) if chroma else range(1))}
+    want |= {("bdpcm", (m, w, h)) for m in (abi.INTRA_BDPCM_HOR, abi.INTRA_BDPCM_VER) for (w, h) in luma if w <= 32 and h <= 32}
+    assert len([t for t in want if t[0] == "cubic_lo"]) >= len(luma) * 2
+    assert want <= got, sorted(want - got)
+    assert {t for t, _ in got} == set(synth.INTRA_TARGETS)
+    if "stride" in name: assert all(s % 2 for s in case["g"].stride)
+    if "yuv400" in name: assert case["g"].chromaFormat == 0 and (case["recs"]["comp"] == 0).all()
+    _rules_accept(case)
+
+
+@pytest.mark.parametrize("name", [n for n, v in synth.INTRA_SWEEP_CASES.items() if v[0] == "flat"])
+def test_intra_flat_predicts_its_value(oracle, name):
+    """Every block of a flat case predicts its value v in every sample, for each v in {0, 1, mid, pmax - 1, pmax}, with full and cut neighbourhoods,
+    through planar, DC, every angular mode on every shape, MRL 1 and 2, BDPCM; the angular modes take both the cubic and the Gaussian filter, and the
+    filtered reference."""
+    case = synth.intra_designed_sweep(name)
+    bd, recs = case["bd"], case["recs"]
+    probes = helpers.intra_probes(oracle, case["g"], case["planes"], recs)
+    seen, interp = set(), {}
+    for r, v, p in zip(recs, case["flat"], probes):
+        assert (p.predMin, p.predMax) == (v, v), (r, v, p.predMin, p.predMax)
+        c, w, h, m = int(r["comp"]), 1 << int(r["log2w"]), 1 << int(r["log2h"]), int(r["mode"])
+        seen.add((c, w, h, m, int(r["multiRefIdx"])))
+        interp.setdefault(m, set()).add(p.interp + 4 * p.filtered)
+    pmax = (1 << bd) - 1
+    assert set(case["flat"]) == {0, 1, 1 << (bd - 1), pmax - 1, pmax}
+    for c, shapes in ((0, synth.INTRA_LUMA_SHAPES), (1, synth.INTRA_CHROMA_SHAPES), (2, synth.INTRA_CHROMA_SHAPES)):
+        for (w, h) in shapes:
+            assert all((c, w, h, m, 0) in seen for m in range(67)), (c, w, h)
+            if c == 0: assert {mrl for (cc, ww, hh, m, mrl) in seen if (cc, ww, hh) == (0, w, h)} == ({0, 1, 2} if h < case["ctu"] else {0})
+            if c == 0 and w <= 32 and h <= 32: assert {(0, w, h, abi.INTRA_BDPCM_HOR, 0), (0, w, h, abi.INTRA_BDPCM_VER, 0)} <= seen
+    assert sum(1 for m in range(2, 67) if {1, 2} <= interp[m]) > 50           # most angular modes take both filters (on different shapes)
+    assert any(5 in interp[m] or 4 in interp[m] for m in range(2, 67))       # angular modes on the filtered reference
+    assert {(int(r["numAbove"]) < 2 * (1 << int(r["log2w"])) // (2 if r["comp"] else 4)) for r in recs} == {False, True}
+    _rules_accept(case)
+
+
+@pytest.mark.parametrize("name", [n for n in synth.INTRA_SWEEP_CASES if n != "regular_chained"])
+def test_intra_designed_cases_are_independent_and_in_ctu_order(name):
+    """No block's reference footprint (4 luma / 2 chroma rows above from the corner to 2w, as many columns left down to 2h) holds another block's
+    samples; records are in CTU raster order, every block inside its CTU, MRL never on the first row of a CTU."""
+    case = synth.intra_designed_sweep(name)
+    recs, W, H, ctu = case["recs"], case["W"], case["H"], case["ctu"]
+    key = ((recs["y"].astype(np.int64) << (recs["comp"] > 0)) // ctu) * (W // ctu) + ((recs["x"].astype(np.int64) << (recs["comp"] > 0)) // ctu)
+    assert np.all(np.diff(key) >= 0)
+    assert not (recs["y"][recs["multiRefIdx"] > 0] % ctu == 0).any()
+    for c in range(3 if case["planes"][1] is not None else 1):
+        r = recs[recs["comp"] == c]
+        gap, cs, pw, ph = (2, ctu // 2, W // 2, H // 2) if c else (4, ctu, W, H)
+        occ = np.zeros((ph, pw), bool)
+        for t in r:
+            x, y, w, h = int(t["x"]), int(t["y"]), 1 << int(t["log2w"]), 1 << int(t["log2h"])
+            assert x // cs == (x + w - 1) // cs and y // cs == (y + h - 1) // cs
+            assert not occ[y:y + h, x:x + w].any()
+            occ[y:y + h, x:x + w] = True
+        for t in r:
+            x, y, w, h = int(t["x"]), int(t["y"]), 1 << int(t["log2w"]), 1 << int(t["log2h"])
+            assert x + 2 * w <= pw and y + 2 * h <= ph
+            assert not occ[max(0, y - gap):y, max(0, x - gap):x + 2 * w].any() and not occ[max(0, y - gap):y + 2 * h, max(0, x - gap):x].any(), (c, x, y, w, h)
+
+
+def test_intra_chained_depends_on_its_producers(oracle):
+    """The chained case: leaving out any one producer changes its consumer's prediction (the last above-right unit, the last below-left unit, the
+    corner, MRL line 2); producers sit in the CTU above, the CTU to the left, the CTU above-right, the CTU above-left and the consumer's own CTU."""
+    case = synth.intra_designed_sweep("regular_chained")
+    g, recs, planes, tags, ctu = case["g"], case["recs"], case["planes"], case["tags"], case["ctu"]
+    full = [p.copy() for p in planes]
+    oracle.orc_intra_predict(C.byref(g), abi.plane_ptrs(full), recs.ctypes.data, len(recs))
+    where = set()
+    for i, tag in enumerate(tags):
+        if tag[0] != "producer": continue
+        j = tags.index(("consumer",) + tag[1:])
+        assert j > i
+        cons, prod = recs[j], recs[i]
+        less = np.ascontiguousarray(np.delete(recs, i))
+        got = [p.copy() for p in planes]
+        oracle.orc_intra_predict(C.byref(g), abi.plane_ptrs(got), less.ctypes.data, len(less))
+        x, y, w, h = int(cons["x"]), int(cons["y"]), 1 << int(cons["log2w"]), 1 << int(cons["log2h"])
+        assert not np.array_equal(got[0][y:y + h, x:x + w], full[0][y:y + h, x:x + w]), tag
+        where.add((tag[1], (int(prod["x"]) // ctu - x // ctu, int(prod["y"]) // ctu - y // ctu)))
+    owner = np.full(planes[0].shape, len(recs))                      # no block claims a neighbour that a later block writes (a decoding order)
+    for i, t in enumerate(recs): owner[int(t["y"]):int(t["y"]) + (1 << int(t["log2h"])), int(t["x"]):int(t["x"]) + (1 << int(t["log2w"]))] = i
+    for i, t in enumerate(recs):
+        x, y, m, na, nl = int(t["x"]), int(t["y"]), int(t["multiRefIdx"]), 4 * int(t["numAbove"]), 4 * int(t["numLeft"])
+        reads = np.concatenate([owner[y - 1 - m:y, x:x + na].ravel(), owner[y:y + nl, x - 1 - m:x].ravel(), owner[y - 1 - m:y, x - 1 - m:x].ravel()])
+        assert not ((reads > i) & (reads < len(recs))).any(), i
+    assert {d for _, d in where} == {(1, -1), (-1, 0), (-1, -1), (0, -1), (0, 0)}
+    assert {t for t, _ in where} == {"above_right", "below_left", "corner", "above", "mrl2"}
+    assert (recs["multiRefIdx"] == 2).any() and not (recs["y"][recs["multiRefIdx"] > 0] % ctu == 0).any()
+    _rules_accept(case)

@@ -103,8 +103,8 @@ def test_intra_predict_only_and_golden(b200):
 
 @functools.lru_cache(maxsize=None)
 def _sweep(reconstruct, name="modes"):
-    if name != "modes":                                           # a case of the designed CCLM sweep: its own planes and residual
-        case = synth.cclm_sweep(name)
+    if name != "modes":                                           # a case of the designed CCLM or regular sweep: its own planes and residual
+        case = synth.intra_designed_sweep(name) if name in synth.INTRA_SWEEP_CASES else synth.cclm_sweep(name)
         g, planes, recs = case["g"], case["planes"], case["recs"]
         resi = case["resi"] if reconstruct else None
         return g, planes, resi, recs, _reconstruct(g, planes, resi, recs)
@@ -118,15 +118,23 @@ def _sweep(reconstruct, name="modes"):
 
 @pytest.mark.parametrize("kernel", INTRA_KERNELS)
 @pytest.mark.parametrize("reconstruct", [False, True], ids=["predict", "reconstruct"])
-@pytest.mark.parametrize("name", ["modes"] + list(synth.CCLM_SWEEP_CASES))
+@pytest.mark.parametrize("name", ["modes"] + list(synth.CCLM_SWEEP_CASES) + list(synth.INTRA_SWEEP_CASES))
 def test_intra_designed_sweep(b200, kernel, reconstruct, name):
     """modes: every (component, shape, mode) combination K6 takes, MRL, BDPCM and every MIP mode, each with a full, a partial and no neighbourhood, on
     noise.  The CCLM cases (synth.CCLM_SWEEP_CASES): every chroma shape and LM / MDLM neighbourhood under each luma filter and at the picture edges;
     templates designed to reach every target of the parameter derivation at 8, 10 and 12 bit; CCLM blocks whose templates and co-located luma are
     written by luma blocks before them, in other CTUs.  tests/test_k6_cases_cpu.py checks what each list covers and that no block reads another
-    (except in the chained case)."""
+    (except in the chained case).  The regular cases (synth.INTRA_SWEEP_CASES): references designed so that every clip of the prediction binds below 0
+    and above pmax, substitution, flat references, 8 / 10 / 12 bit, CTU 32 / 64, odd strides, 4:0:0, and blocks whose far reference units are written
+    by blocks before them.  Without a residual, every block of a flat case predicts its value in every sample (checked on the device output alone)."""
     g, planes, resi, recs, want = _sweep(reconstruct, name)
-    assert_planes_equal(intra_run(b200, kernel, g, planes, recs, resi), want, (name, kernel))
+    got = intra_run(b200, kernel, g, planes, recs, resi)
+    assert_planes_equal(got, want, (name, kernel))
+    if name.startswith("regular_flat") and not reconstruct:
+        flat = synth.intra_designed_sweep(name)["flat"]
+        for r, v in zip(recs, flat):
+            x, y, w, h = int(r["x"]), int(r["y"]), 1 << int(r["log2w"]), 1 << int(r["log2h"])
+            assert (got[int(r["comp"])][y:y + h, x:x + w] == v).all(), (name, kernel, r, v)
 
 
 @functools.lru_cache(maxsize=None)

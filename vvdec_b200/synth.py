@@ -1171,9 +1171,11 @@ def _cclm_record(x, y, w, h, comp, nb, colloc):
     return r
 
 
-def _cclm_pack(blocks, C, ctus_w):
-    """Chroma positions of blocks [(w, h, where)] in CTU raster order (size C, ctus_w CTUs a row): the first position on the 2-sample grid inside a
-    CTU where the block's footprint is free.  where: "any"; "first_row" (y on the first row of a CTU below the first); "left_edge" (x = 0); "top_edge" (y = 0)."""
+def _cclm_pack(blocks, C, ctus_w, gap=2):
+    """Positions of blocks [(w, h, where)] in CTU raster order (size C, ctus_w CTUs a row): the first position on the `gap`-sample grid inside a CTU
+    where the block's footprint (its `gap` reference rows / columns in front of it, its 2w x 2h reach) is free.  where: "any" (the first row of a CTU
+    only where nothing else is free); "inner" (never the first row of a CTU: blocks with MRL); "first_row" (y on the first row of a CTU below the first); "left_edge" (x = 0); "top_edge" (y = 0).
+    CCLM packs chroma blocks with gap 2; the regular intra sweep packs luma with gap 4 (MRL 2 reads the third row / column in front of a block)."""
     Wc = C * ctus_w
     occ = np.zeros((C * 128, Wc), bool)
     cursor, out = {}, [None] * len(blocks)
@@ -1182,18 +1184,26 @@ def _cclm_pack(blocks, C, ctus_w):
         k = cursor.get((w, h, where), ctus_w if where == "first_row" else 0)
         while True:
             cx, cy = (k % ctus_w) * C, (k // ctus_w) * C
-            xs = [x for x in range(cx, cx + C - w + 1, 2) if x >= 2]
-            ys = [y for y in list(range(cy + 2, cy + C - h + 1, 2)) + [cy] if y >= 2]    # the first row of a CTU last: only a block as high as the CTU sits there
+            xs = [x for x in range(cx, cx + C - w + 1, gap) if x >= gap]
+            ys = [y for y in list(range(cy + gap, cy + C - h + 1, gap)) + [cy] if y >= gap]    # the first row of a CTU last: only a block as high as the CTU sits there
             slots = [(x, y) for y in ys for x in xs]
-            cands = {"any": slots, "first_row": [(x, cy) for x in xs], "left_edge": [(0, y) for y in ys] if cx == 0 else [],
+            cands = {"any": slots, "inner": [(x, y) for (x, y) in slots if y != cy], "first_row": [(x, cy) for x in xs], "left_edge": [(0, y) for y in ys] if cx == 0 else [],
                      "top_edge": [(x, 0) for x in xs] if cy == 0 else []}[where]
-            hit = next(((x, y) for (x, y) in cands if x + 2 * w <= Wc and not occ[max(0, y - 2):y + 2 * h, max(0, x - 2):x + 2 * w].any()), None)
-            if hit: break
+            cands = [(x, y) for (x, y) in cands if x + 2 * w <= Wc]
+            if cands:                                                # the footprint sums of all candidates at once, from an integral image of the CTU's window
+                X, Y = np.array(cands).T
+                wx, wy = max(0, cx - gap), max(0, cy - gap)
+                win = occ[wy:cy + C + 2 * h, wx:cx + C + 2 * w]
+                ii = np.zeros((win.shape[0] + 1, win.shape[1] + 1), np.int32)
+                ii[1:, 1:] = win.cumsum(0).cumsum(1)
+                y0, y1, x0, x1 = np.maximum(0, Y - gap) - wy, Y + 2 * h - wy, np.maximum(0, X - gap) - wx, X + 2 * w - wx
+                free = np.flatnonzero(ii[y1, x1] - ii[y0, x1] - ii[y1, x0] + ii[y0, x0] == 0)
+                if len(free): hit = cands[free[0]]; break
             k += 1
             assert where != "top_edge" or k < ctus_w, "the top edge is full"
         cursor[(w, h, where)] = k
         x, y = hit
-        occ[max(0, y - 2):y + 2 * h, max(0, x - 2):x + 2 * w] = True
+        occ[max(0, y - gap):y + 2 * h, max(0, x - gap):x + 2 * w] = True
         out[i] = hit
     return out
 
@@ -1337,6 +1347,214 @@ def cclm_sweep(name):
     resi = [rng.integers(-64, 65, size=p.shape).astype(np.int16) for p in planes]
     case = dict(name=name, g=g, W=W, H=H, bd=bd, ctu=ctu, planes=planes, resi=resi, recs=recs, tags=tags)
     _cclm_sweep_cache[name] = case
+    return case
+
+
+# ---------------------------------------------------------------------------------------------------------------- designed regular intra sweep
+# Regular intra records (planar, DC, angular, MRL, PDPC, BDPCM, MIP) on designed reference samples, as named cases (tests/test_k6_*.py):
+#   regular_targets_{8,10,12}bit: each block's reference rows and columns are written so that a clip site of the prediction sees values below 0 and above
+#     pmax (INTRA_TARGETS: the cubic interpolation of fractional luma angles with MRL 0, 1 and 2, PDPC of modes 18 and 50, the reduced MIP prediction
+#     of each size class, transposed and not), substitution takes the mid value (no neighbour) or pads from one available unit at 0 or pmax, BDPCM
+#     copies references at 0 and pmax; the residual is large enough that pred + resi crosses 0 and pmax in every component.
+#   regular_flat_{8,12}bit: every reference sample (MRL lines included) of a block holds one value v in {0, 1, mid, pmax - 1, pmax}, with full and partial
+#     neighbourhoods: planar, DC, every angular mode, MRL 1 and 2 (every third angular mode), BDPCM on every shape.  Every predicted sample is v (MIP is left out: its output on
+#     flat input is not v).
+#   regular_geometry_ctu{32,64}: the targets blocks of every shape that fits the CTU (8 and 12 bit), blocks without a neighbour also at the picture's
+#     top and left edges; regular_stride_odd_12bit: the same at CTU 128 on planes with odd, padded strides (the one-CTA-per-block path);
+#     regular_yuv400_10bit: luma only (CTU 64).
+#   regular_chained: consumer blocks whose last above-right unit, last below-left unit, corner and MRL line 2 are written by earlier producer blocks, in the
+#     CTU above, the CTU to the left, the CTU above-right and the CTU itself, at 12 bit with producers at 0 and pmax.
+# Every block owns its footprint: its reference rows / columns (4 luma, 2 chroma: MRL lines included), its 2w / 2h reach and its corner.  Footprints
+# never overlap (except in the chained case), so no block reads another block's samples.
+INTRA_LUMA_SHAPES = tuple((w, h) for w in (4, 8, 16, 32, 64) for h in (4, 8, 16, 32, 64))
+INTRA_CHROMA_SHAPES = tuple((w, h) for w in (4, 8, 16, 32) for h in (4, 8, 16, 32))
+INTRA_TARGETS = ("cubic_lo", "cubic_hi", "pdpc_lo", "pdpc_hi", "mip_lo", "mip_hi", "subst_mid", "pad_0", "pad_max", "reco_lo", "reco_hi", "bdpcm")
+INTRA_SWEEP_CASES = {
+    "regular_targets_8bit": ("targets", 128, 8, None, True), "regular_targets_10bit": ("targets", 128, 10, None, True), "regular_targets_12bit": ("targets", 128, 12, None, True),
+    "regular_flat_8bit": ("flat", 128, 8, None, True), "regular_flat_12bit": ("flat", 128, 12, None, True),
+    "regular_geometry_ctu32": ("targets", 32, 8, None, True), "regular_geometry_ctu64": ("targets", 64, 12, None, True),
+    "regular_stride_odd_12bit": ("targets", 128, 12, 7, True), "regular_yuv400_10bit": ("targets", 64, 10, None, False),
+    "regular_chained": ("chained", 64, 12, None, True),
+}
+
+
+def intra_mip_modes(w, h):
+    """Number of MIP modes of a w x h luma block's size class (getMipSizeId: 4x4; 4xN, Nx4 and 8x8; the rest)."""
+    return 16 if (w, h) == (4, 4) else 8 if (w == 4 or h == 4 or (w, h) == (8, 8)) else 6
+
+
+def intra_cubic_modes(w, h, mrl):
+    """Up to three angular modes of a w x h luma block that interpolate a fractional angle with the cubic filter: with MRL every fractional angle
+    does; without it only angles close enough to horizontal / vertical for the block size (intra_filter_ref's threshold).  Spread over the range."""
+    out = []
+    for m in range(2, 67):
+        pm = intra_wide_angle(w, h, m)
+        a = _INTRA_ANG[abs(pm - 50 if pm >= 34 else -(pm - 18))]
+        diff = min(abs(pm - 18), abs(pm - 50))
+        if a & 31 and (mrl or diff <= _INTRA_THR[(int(np.log2(w)) + int(np.log2(h))) >> 1]): out.append(m)
+    return [out[i] for i in sorted({0, len(out) // 2, len(out) - 1})] if out else []
+
+
+def _intra_pattern(kind, bd, v=0):
+    """pattern(k, n, left): the value of reference sample k of a block whose side is n samples long (k = 0: the corner, k >= 1: the k-th sample of the
+    row above, or of the column to the left, k < 0: the MRL corner)."""
+    pmax, mid = (1 << bd) - 1, 1 << (bd - 1)
+    return {"cubic": lambda k, n, l: pmax if (k // 2) % 2 else 0,                 # 0 0 pmax pmax 0 0 ...: 4-tap windows across a step overshoot
+            "pdpc": lambda k, n, l: mid if k <= 0 else pmax if k % 2 else 0,      # corner mid, sides pmax 0 pmax ...: pmax + (pmax - mid) / 2 and -mid * wL / 64
+            "bdpcm": lambda k, n, l: pmax if k % 2 else 0,
+            "mip_a": lambda k, n, l: mid if k <= 0 else (pmax if k <= n // 2 else 0) ^ (pmax if l else 0),   # above: pmax then 0; left: 0 then pmax
+            "mip_b": lambda k, n, l: mid if k <= 0 else (0 if k <= n // 2 else pmax) ^ (pmax if l else 0),
+            "flat": lambda k, n, l: v, "pad": lambda k, n, l: v}[kind]
+
+
+def _intra_paint(plane, x, y, w, h, gap, pattern):
+    """Writes a block's reference footprint: `gap` identical rows above (corner, then 2w samples) and `gap` identical columns to the left (corner,
+    then 2h samples); the MRL corner samples continue the pattern at k < 0."""
+    top = np.array([pattern(k, w, 0) for k in range(1 - gap, 2 * w + 1)], np.int16)
+    left = np.array([pattern(k, h, 1) for k in range(1 - gap, 2 * h + 1)], np.int16)
+    x0, y0 = max(0, x - gap), max(0, y - gap)                      # at the picture's edges only the part inside the picture
+    for d in range(gap):
+        if y - 1 - d >= 0: row = plane[y - 1 - d, x0:x + 2 * w]; row[:] = top[x0 - x + gap:][:len(row)]
+        if x - 1 - d >= 0: col = plane[y0:y + 2 * h, x - 1 - d]; col[:] = left[y0 - y + gap:][:len(col)]
+    plane[y0:y, x0:x] = pattern(0, 0, 0)
+
+
+def _intra_targets_blocks(C, chroma):
+    """(comp, w, h, mode, mrl, mip, nb, pattern, v, where) of a targets case with luma CTU size C: cubic modes with MRL 0 / 1 / 2 on every luma shape
+    (MRL never on a block as high as the CTU: it could only sit on the CTU's first row), modes 18 / 50 on every shape (PDPC), every MIP mode of every
+    shape, transposed and not, BDPCM H / V up to 32x32; per shape a block without neighbours and blocks padded from one unit at 0 and at pmax, and
+    one more at the picture's top edge (no neighbour, or the unit left) and one at its left edge (no neighbour, or the unit above), alternating by shape."""
+    A = abi
+    out = []
+    shapes = [(k, 0, w, h) for k, (w, h) in enumerate(INTRA_LUMA_SHAPES) if w <= C and h <= C]
+    if chroma: shapes += [(k, c, w, h) for c in (1, 2) for k, (w, h) in enumerate(INTRA_CHROMA_SHAPES) if w <= C // 2 and h <= C // 2]
+    for (k, c, w, h) in shapes:                                      # Cr repeats the blocks of Cb: it takes their positions, in its own plane
+        if c == 0:
+            for mrl in (0, 1, 2):
+                if mrl and h == C: continue
+                out += [(c, w, h, m, mrl, 0, "full", "cubic", 0, "inner" if mrl else "any") for m in intra_cubic_modes(w, h, mrl)]
+            out += [(c, w, h, A.INTRA_MIP, 0, m | (tr << 7), "full", p, 0, "any") for m in range(intra_mip_modes(w, h)) for tr in (0, 1) for p in ("mip_a", "mip_b")]
+            if w <= 32 and h <= 32: out += [(c, w, h, m, 0, 0, "full", "bdpcm", 0, "any") for m in (A.INTRA_BDPCM_HOR, A.INTRA_BDPCM_VER)]
+        out += [(c, w, h, m, 0, 0, "full", "pdpc", 0, "any") for m in (18, 50)]
+        out += [(c, w, h, (1, 66, 2)[k % 3], 0, 0, "none", None, 0, "any"),
+                (c, w, h, 50, 0, 0, "one_above", "pad", "0", "any"), (c, w, h, 18, 0, 0, "one_left", "pad", "max", "any"),
+                (c, w, h, 1, 0, 0, "one_above", "pad", "max", "any"), (c, w, h, 0, 0, 0, "one_left", "pad", "0", "any")]
+        out += [(c, w, h, 0, 0, 0, "none", None, 0, "top_edge") if k & 1 else (c, w, h, 66, 0, 0, "one_left", "pad", "max", "top_edge"),
+                (c, w, h, 1, 0, 0, "none", None, 0, "left_edge") if k & 1 else (c, w, h, 2, 0, 0, "one_above", "pad", "0", "left_edge")]
+    return out
+
+
+def _intra_flat_blocks(C, chroma):
+    """(comp, w, h, mode, mrl, mip, nb, pattern, v, where) of a flat case: every shape with planar, DC, every angular mode, MRL 1 and 2 with every
+    third angular mode (luma), BDPCM H / V (luma up to 32x32); v and the neighbourhood (full, above-right cut, below-left cut) rotate over the blocks."""
+    A = abi
+    out = []
+    shapes = [(0, w, h) for (w, h) in INTRA_LUMA_SHAPES if w <= C and h <= C]
+    if chroma: shapes += [(c, w, h) for c in (1, 2) for (w, h) in INTRA_CHROMA_SHAPES if w <= C // 2 and h <= C // 2]
+    for (c, w, h) in shapes:
+        ms = [(m, 0) for m in range(67)]
+        if c == 0: ms += [(m, mrl) for mrl in (1, 2) for m in range(1 + mrl, 67, 3) if h < C] + ([(A.INTRA_BDPCM_HOR, 0), (A.INTRA_BDPCM_VER, 0)] if w <= 32 and h <= 32 else [])
+        for i, (m, mrl) in enumerate(ms):
+            out.append((c, w, h, m, mrl, 0, ("full", "cut_above", "cut_left")[i % 3], "flat", ("0", "1", "mid", "max-1", "max")[(i + w + h) % 5], "inner" if mrl else "any"))
+    return out
+
+
+def _intra_value(v, bd):
+    pmax = (1 << bd) - 1
+    return {"0": 0, "1": 1, "mid": 1 << (bd - 1), "max-1": pmax - 1, "max": pmax}[v] if isinstance(v, str) else v
+
+
+def _intra_record(c, x, y, w, h, mode, mrl, mip, nb):
+    A = abi
+    unit = 2 if c else 4
+    r = np.zeros((), A.INTRA_TU_DTYPE)
+    r["x"], r["y"], r["log2w"], r["log2h"], r["comp"], r["mode"], r["multiRefIdx"], r["mip"] = x, y, int(np.log2(w)), int(np.log2(h)), c, mode, mrl, mip
+    na, nl = {"full": (2 * w // unit, 2 * h // unit), "cut_above": (w // unit, 2 * h // unit), "cut_left": (2 * w // unit, h // unit),
+              "none": (0, 0), "one_above": (1, 0), "one_left": (0, 1)}[nb]
+    fl = A.INTRA_ADD_RESI | (A.INTRA_AVAIL_TL if nb == "full" else 0)
+    if c == 0 and mode <= 66 and intra_filter_ref(w, h, mode, mrl, 0): fl |= A.INTRA_FILTER_REF
+    r["flags"], r["numAbove"], r["numLeft"] = fl, na, nl
+    return r
+
+
+def _intra_chained(ctu, bd):
+    """Consumers at CTU (k + 1, 1), k = 0..n - 1, each 16x16 unless noted, each after the producer that writes one of its far reference units, every
+    producer a 4x4 (8x4) DC block whose own references are flat at 0 or pmax (its below-left unit is not available): mode 34 at the CTU's top-left corner, its corner in the CTU above-left;
+    mode 66 at the top of the CTU, its last above-right unit in the CTU above; mode 66 at the CTU's top right, its last above-right unit in the CTU
+    above-right; mode 2 at the CTU's left edge, its last below-left unit in the CTU to the left; an 8x8 mode 45 block with MRL 2 inside the CTU, its
+    three reference rows written by an 8x4 producer of the same CTU.  Tags: (role, what, k)."""
+    A = abi
+    n_ctu = 4
+    W, H = (n_ctu + 2) * ctu, 3 * ctu
+    recs, tags = [], []
+    paints = []                                                   # (x, y, w, h, value) of each producer's reference footprint
+    for k in range(n_ctu):
+        X, Y = (k + 1) * ctu, ctu
+        v = (k & 1) * ((1 << bd) - 1)
+        cons = [(X, Y, 16, 16, 34, 0, "corner"), (X + 24, Y, 16, 16, 66, 0, "above"), (X + ctu - 16, Y, 16, 16, 66, 0, "above_right"),
+                (X, Y + 16, 16, 16, 2, 0, "below_left"), (X + 48, Y + 24, 8, 8, 45, 2, "mrl2")]      # in decoding order: no block reads a later one
+        prods = {"above_right": [(X + ctu + 12, Y - 4, 4, 4)], "below_left": [(X - 4, Y + 44, 4, 4)], "corner": [(X - 4, Y - 4, 4, 4)],
+                 "above": [(X + 52, Y - 4, 4, 4)], "mrl2": [(X + 48, Y + 20, 8, 4)]}
+        for (x, y, w, h, mode, mrl, what) in cons:
+            for (px, py, pw, ph) in prods[what]:
+                pv = ((1 << bd) - 1) - v if what in ("corner", "mrl2") else v
+                r = _intra_record(0, px, py, pw, ph, 1, 0, 0, "cut_left")     # its below-left is a later block: not available
+                recs.append(r); tags.append(("producer", what, k)); paints.append((px, py, pw, ph, pv))
+            recs.append(_intra_record(0, x, y, w, h, mode, mrl, 0, "full")); tags.append(("consumer", what, k))
+    recs = np.array(recs, A.INTRA_TU_DTYPE)
+    key = (recs["y"].astype(int) // ctu) * (W // ctu) + recs["x"].astype(int) // ctu
+    order = np.argsort(key, kind="stable")
+    return W, H, recs[order], [tags[i] for i in order], paints
+
+
+_intra_sweep_cache = {}
+
+
+def intra_designed_sweep(name):
+    """One case of the designed regular intra sweep (INTRA_SWEEP_CASES) as a dict: geometry (g, W, H, bd, ctu), noise planes with the designed
+    references written in (planes; Cb / Cr None in 4:0:0), the residual planes (resi), the records in CTU order (recs) and per record what it was built
+    for (tags: (pattern, value, neighbourhood, where), or the chained role); flat: the value every predicted sample of a record must hold (-1: none)."""
+    if name in _intra_sweep_cache: return _intra_sweep_cache[name]
+    kind, ctu, bd, pad, chroma = INTRA_SWEEP_CASES[name]
+    rng = np.random.default_rng(sum(map(ord, name)))
+    pmax = (1 << bd) - 1
+    if kind == "chained":
+        W, H, recs, tags, paints = _intra_chained(ctu, bd)
+        planes = noise_planes(rng, W, H, bd)
+        for (x, y, w, h, v) in paints: _intra_paint(planes[0], x, y, w, h, 4, _intra_pattern("flat", bd, v))
+        flat = np.full(len(recs), -1)
+    else:
+        blocks = _intra_targets_blocks(ctu, chroma) if kind == "targets" else _intra_flat_blocks(ctu, chroma)
+        ctus_w = max(8, 2048 // ctu)
+        luma = [i for i, b in enumerate(blocks) if b[0] == 0]
+        cb = [i for i, b in enumerate(blocks) if b[0] == 1]
+        cr = [i for i, b in enumerate(blocks) if b[0] == 2]
+        pos = {}
+        for i, p in zip(luma, _cclm_pack([(blocks[i][1], blocks[i][2], blocks[i][9]) for i in luma], ctu, ctus_w, gap=4)): pos[i] = p
+        for i, p in zip(cb, _cclm_pack([(blocks[i][1], blocks[i][2], blocks[i][9]) for i in cb], ctu // 2, ctus_w, gap=2)): pos[i] = p
+        for i, j in zip(cr, cb): pos[i] = pos[j]                  # Cr blocks sit where the Cb blocks of the same list position sit, in their own plane
+        assert all(blocks[i][1:3] == blocks[j][1:3] for i, j in zip(cr, cb))
+        W = ctus_w * ctu
+        H = ((max((y + 2 * blocks[i][2]) << (blocks[i][0] > 0) for i, (x, y) in pos.items()) + ctu - 1) // ctu + 1) * ctu
+        strides = (W + pad, W // 2 + pad, W // 2 + pad) if pad else None
+        planes = noise_planes(rng, W, H, bd, chroma=chroma, strides=strides)
+        per = []
+        for i, b in enumerate(blocks):
+            c, w, h, mode, mrl, mip, nb, pattern, v, where = b
+            x, y = pos[i]
+            if pattern: _intra_paint(planes[c], x, y, w, h, 2 if c else 4, _intra_pattern(pattern, bd, _intra_value(v, bd)))
+            per.append((_intra_record(c, x, y, w, h, mode, mrl, mip, nb), (pattern, v, nb, where), _intra_value(v, bd) if pattern == "flat" else -1))
+        key = [((int(r["y"]) << (r["comp"] > 0)) // ctu) * (W // ctu) + ((int(r["x"]) << (r["comp"] > 0)) // ctu) for r, _, _ in per]
+        order = np.argsort(key, kind="stable")
+        recs = np.array([per[i][0] for i in order], abi.INTRA_TU_DTYPE)
+        tags = [per[i][1] for i in order]
+        flat = np.array([per[i][2] for i in order])
+    g = abi.make_geom(W, H, bd, chroma_format=1 if chroma else 0, ctu=ctu, strides=tuple(p.shape[1] for p in planes) if chroma else (planes[0].shape[1], 0, 0))
+    lim = (3 * pmax) // 4 if kind != "flat" else 64
+    resi = [rng.integers(-lim, lim + 1, size=p.shape).astype(np.int16) for p in planes]
+    if not chroma: planes, resi = planes + [None, None], resi + [None, None]
+    case = dict(name=name, g=g, W=W, H=H, bd=bd, ctu=ctu, planes=planes, resi=resi, recs=recs, tags=tags, flat=flat)
+    _intra_sweep_cache[name] = case
     return case
 
 
