@@ -35,6 +35,32 @@ void set_error(const char* fmt, ...);
 __device__ __forceinline__ int clip3(int lo, int hi, int v) { return min(max(v, lo), hi); }
 __device__ __forceinline__ int clip16(int v) { return min(max(v, -32768), 32767); }
 
+// Four int16 samples as one 8-byte word pair (K4 and K5 move 4 samples per thread)
+__device__ __forceinline__ void unpack4(const uint2 u, int* d) { d[0] = (int)(int16_t)(u.x & 0xffff); d[1] = (int)(int16_t)(u.x >> 16); d[2] = (int)(int16_t)(u.y & 0xffff); d[3] = (int)(int16_t)(u.y >> 16); }
+__device__ __forceinline__ uint2 pack4(const int* v)
+{
+  uint2 o;
+  o.x = (unsigned)(v[0] & 0xffff) | ((unsigned)v[1] << 16);
+  o.y = (unsigned)(v[2] & 0xffff) | ((unsigned)v[3] << 16);
+  return o;
+}
+
+// Asynchronous global -> shared copies of 4, 8 and 16 bytes (LDGSTS): a CTA issues its whole footprint without waiting on any load, then waits once.
+// 16-byte copies bypass L1 (.cg); the smaller sizes only exist cached (.ca).
+__device__ __forceinline__ void cp_async4(void* smemDst, const void* gmemSrc)
+{
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" :: "r"((unsigned)__cvta_generic_to_shared(smemDst)), "l"(gmemSrc));
+}
+__device__ __forceinline__ void cp_async8(void* smemDst, const void* gmemSrc)
+{
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" :: "r"((unsigned)__cvta_generic_to_shared(smemDst)), "l"(gmemSrc));
+}
+__device__ __forceinline__ void cp_async16(void* smemDst, const void* gmemSrc)
+{
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"((unsigned)__cvta_generic_to_shared(smemDst)), "l"(gmemSrc));
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+
 // LMCS forward map of one predicted luma sample (rspFwdCore, reference CommonLib/Buffer.cpp:321); L points at the uploaded b200_lmcs
 __device__ __forceinline__ int lmcs_fwd(const b200_lmcs* __restrict__ L, int log2OrgCW, int v, int pmax)
 {

@@ -39,14 +39,6 @@ struct McParams {
   const b200_lmcs* lmcs; int lmcsLog2;       // LMCS: luma predictions are stored forward-mapped (DecCu.cpp:458-476); null = off
 };
 
-// asynchronous 4-byte global -> shared copies (LDGSTS): a tile issues its whole footprint without waiting on any load, then waits once
-__device__ __forceinline__ void cp_async4(void* smemDst, const void* gmemSrc)
-{
-  const unsigned d = (unsigned)__cvta_generic_to_shared(smemDst);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" :: "r"(d), "l"(gmemSrc));
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
-
 // One reference plane seen through an inclusive clamp rectangle: a position outside it reads the nearest sample inside.  The rectangle is
 // the picture (the reference's border extension) or, for DMVR's final MC, the padded window intersected with the picture (xPrefetchPad
 // :1525).  Every per-sample reference read goes through here, on the read-only path.

@@ -263,7 +263,7 @@ int launch_lf_deblock(const LfLaunch& L, cudaStream_t s, KHook* hook)
   LfParams P;
   for (int c = 0; c < 3; c++) { P.plane[c] = L.planes.p[c]; P.stride[c] = L.planes.stride[c]; }
   P.W = L.geom.width; P.H = L.geom.height; P.W4 = (P.W + 3) >> 2; P.H4 = (P.H + 3) >> 2;
-  P.bitDepth = L.geom.bitDepth; P.ctuSize = L.geom.ctuSize; P.ctuLog2 = L.geom.ctuSize == 128 ? 7 : L.geom.ctuSize == 64 ? 6 : 5;
+  P.bitDepth = L.geom.bitDepth; P.ctuSize = L.geom.ctuSize; P.ctuLog2 = ctu_log2(L.geom);
   P.ctusW = (P.W + P.ctuSize - 1) >> P.ctuLog2; P.chroma = L.geom.chromaFormat == 1;
   P.ctuSlice = L.ctuSlice; P.seq = L.seq;
   dim3 blk(32, 8), grd((P.W4 + 31) / 32, (P.H4 + 7) / 8);

@@ -39,7 +39,8 @@ __global__ void __launch_bounds__(256) sao_kernel(const SaoParams P)
   const uint8_t* ob = rec + 6 + c * 5;
   const uint32_t offLo = __ldg(ob) | (__ldg(ob + 1) << 8) | (__ldg(ob + 2) << 16) | (__ldg(ob + 3) << 24), offHi = __ldg(ob + 4);
   auto offset_of = [&](int k) -> int { return (int)(int8_t)__byte_perm(offLo, offHi, k); };
-  int v[4] = { (int)(int16_t)(ctr.x & 0xffff), (int)(int16_t)(ctr.x >> 16), (int)(int16_t)(ctr.y & 0xffff), (int)(int16_t)(ctr.y >> 16) };
+  int v[4];
+  unpack4(ctr, v);
   int r[4] = { v[0], v[1], v[2], v[3] };
   const int pmax = (1 << P.bitDepth) - 1;
   if (type == B200_SAO_BO) {
@@ -68,8 +69,8 @@ __global__ void __launch_bounds__(256) sao_kernel(const SaoParams P)
         na[0] = l; na[1] = v[0]; na[2] = v[1]; na[3] = v[2]; nb[0] = v[1]; nb[1] = v[2]; nb[2] = v[3]; nb[3] = r4;
       } else {
         const uint2 ua = *reinterpret_cast<const uint2*>(rowA + x), ub = *reinterpret_cast<const uint2*>(rowB + x);
-        const int A[4] = { (int)(int16_t)(ua.x & 0xffff), (int)(int16_t)(ua.x >> 16), (int)(int16_t)(ua.y & 0xffff), (int)(int16_t)(ua.y >> 16) };
-        const int B[4] = { (int)(int16_t)(ub.x & 0xffff), (int)(int16_t)(ub.x >> 16), (int)(int16_t)(ub.y & 0xffff), (int)(int16_t)(ub.y >> 16) };
+        int A[4], B[4];
+        unpack4(ua, A); unpack4(ub, B);
         if (dx == 0)      { na[0] = A[0]; na[1] = A[1]; na[2] = A[2]; na[3] = A[3]; nb[0] = B[0]; nb[1] = B[1]; nb[2] = B[2]; nb[3] = B[3]; }
         else if (dx == 1) { na[0] = rowA[xl]; na[1] = A[0]; na[2] = A[1]; na[3] = A[2]; nb[0] = B[1]; nb[1] = B[2]; nb[2] = B[3]; nb[3] = rowB[xr]; }
         else              { na[0] = A[1]; na[1] = A[2]; na[2] = A[3]; na[3] = rowA[xr]; nb[0] = rowB[xl]; nb[1] = B[0]; nb[2] = B[1]; nb[3] = B[2]; }
@@ -109,10 +110,7 @@ __global__ void __launch_bounds__(256) sao_kernel(const SaoParams P)
       if (okMask & (1u << i)) r[i] = clip3(0, pmax, v[i] + offset_of(e + 2));
     }
   }
-  uint2 o;
-  o.x = (unsigned)(r[0] & 0xffff) | ((unsigned)r[1] << 16);
-  o.y = (unsigned)(r[2] & 0xffff) | ((unsigned)r[3] << 16);
-  *dptr = o;
+  *dptr = pack4(r);
 }
 
 int launch_sao(const SaoLaunch& L, cudaStream_t s, KHook* hook)
@@ -120,7 +118,7 @@ int launch_sao(const SaoLaunch& L, cudaStream_t s, KHook* hook)
   SaoParams P;
   for (int c = 0; c < 3; c++) { P.src[c] = L.src.p[c]; P.dst[c] = L.dst.p[c]; P.stride[c] = L.src.stride[c]; }
   P.W = L.geom.width; P.H = L.geom.height; P.bitDepth = L.geom.bitDepth; P.ctuSize = L.geom.ctuSize;
-  P.ctuLog2 = P.ctuSize == 128 ? 7 : P.ctuSize == 64 ? 6 : 5;
+  P.ctuLog2 = ctu_log2(L.geom);
   P.ctusW = (P.W + P.ctuSize - 1) / P.ctuSize; P.chroma = L.geom.chromaFormat == 1;
   P.ctus = L.ctus; P.vb = L.vb;
   dim3 blk(32, 8), grd((P.W / 4 + 31) / 32, (P.H + 7) / 8, P.chroma ? 3 : 1);

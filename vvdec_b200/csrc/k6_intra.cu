@@ -493,18 +493,6 @@ constexpr int V2_FLAGS = 128 * 128 / 16 + 2 * (64 * 64 / 4); // most blocks a CT
 static_assert(V2_FLAGS == INTRA_MAX_CTU_BLOCKS, "the documented per-CTU block limit is the number of done bytes");
 constexpr int V2_OWN = 3 * 32 * 32;                         // owner words of the CTU's units: luma 32 x 32 (4x4 units), Cb / Cr 32 x 32 each (2x2 units)
 constexpr size_t V2_SMEM = (size_t)2 * V2_TILE * sizeof(int16_t) + V2_GROUPS * sizeof(IntraScratch) + V2_RECS * sizeof(b200_intra_tu) + V2_OWN * sizeof(int) + V2_FLAGS + 64;
-__device__ __forceinline__ void v2_cp4(void* smemDst, const void* gmemSrc)      // asynchronous 4-byte global -> shared copy (LDGSTS): the whole CTU in flight before one wait
-{
-  const unsigned d = (unsigned)__cvta_generic_to_shared(smemDst);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" :: "r"(d), "l"(gmemSrc));
-}
-__device__ __forceinline__ void v2_cp16(void* smemDst, const void* gmemSrc)
-{
-  const unsigned d = (unsigned)__cvta_generic_to_shared(smemDst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"(d), "l"(gmemSrc));
-}
-__device__ __forceinline__ void v2_cp_wait() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
-
 __device__ __forceinline__ int v2_tile_off(int c) { return c == 0 ? 0 : c == 1 ? 128 * V2_LS : 128 * V2_LS + 64 * V2_CS; }     // component c in a tile set
 
 // CTUs that hold blocks, sorted by the wave-front key (x + 2 y, then y): every CTU counts the non-empty CTUs that precede it
@@ -606,24 +594,24 @@ __global__ void __launch_bounds__(V2_THREADS, 1) intra_ctu_kernel(const IntraPar
         const int wv = tw >> 3, n = wv * th;
         for (int k = tid; k < n; k += V2_THREADS) {
           const int y = k / wv, x = (k - y * wv) * 8;
-          v2_cp16(rec + y * ts + x, src + (size_t)y * P.stride[c] + x);
-          if (rsrc) v2_cp16(res + y * ts + x, rsrc + (size_t)y * P.stride[c] + x);
+          cp_async16(rec + y * ts + x, src + (size_t)y * P.stride[c] + x);
+          if (rsrc) cp_async16(res + y * ts + x, rsrc + (size_t)y * P.stride[c] + x);
         }
       } else {
         const int wWords = tw >> 1, n = wWords * th;
         for (int k = tid; k < n; k += V2_THREADS) {
           const int y = k / wWords, x = (k - y * wWords) * 2;
-          v2_cp4(rec + y * ts + x, src + (size_t)y * P.stride[c] + x);
-          if (rsrc) v2_cp4(res + y * ts + x, rsrc + (size_t)y * P.stride[c] + x);
+          cp_async4(rec + y * ts + x, src + (size_t)y * P.stride[c] + x);
+          if (rsrc) cp_async4(res + y * ts + x, rsrc + (size_t)y * P.stride[c] + x);
         }
       }
       const int unit = c ? 2 : 4, uw = tw / unit, uh = th / unit;
       const int* osrc = P.owner[c] + (size_t)(oy / unit) * P.ownerStride[c] + ox / unit;
-      for (int k = tid; k < uw * uh; k += V2_THREADS) { const int y = k / uw, x = k - y * uw; v2_cp4(sown + c * 1024 + y * 32 + x, osrc + (size_t)y * P.ownerStride[c] + x); }
+      for (int k = tid; k < uw * uh; k += V2_THREADS) { const int y = k / uw, x = k - y * uw; cp_async4(sown + c * 1024 + y * 32 + x, osrc + (size_t)y * P.ownerStride[c] + x); }
     }
-    for (int k = tid; k < min(cnt, V2_RECS) * 4; k += V2_THREADS) v2_cp4(reinterpret_cast<uint32_t*>(srec) + k, reinterpret_cast<const uint32_t*>(P.tus + first) + k);
+    for (int k = tid; k < min(cnt, V2_RECS) * 4; k += V2_THREADS) cp_async4(reinterpret_cast<uint32_t*>(srec) + k, reinterpret_cast<const uint32_t*>(P.tus + first) + k);
     for (int k = tid; k < cnt; k += V2_THREADS) sflag[k] = P.compSel == 2 ? (uint8_t)(P.tus[first + k].comp == 0) : 0;      // chroma pass: the luma blocks are finished (the pass before)
-    v2_cp_wait();
+    cp_async_wait_all();
     __syncthreads();
 
     // ---- the CTU's blocks, one group each, in decoding order
@@ -712,7 +700,7 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s, KHook* hook)
     for (int c = 0; c < (L.geom.chromaFormat ? 3 : 1); c++) B200_CUDA(cudaMemsetAsync(L.owner[c], 0xff, L.ownerBytes[c], s));
   }
   P.perm = nullptr; P.ctuCnt = P.ctuFirst = P.ctuBase = nullptr;
-  P.ctuLog2 = intra_ctu_log2(L.geom); P.ctusW = (L.geom.width + L.geom.ctuSize - 1) / L.geom.ctuSize; P.ctusH = (L.geom.height + L.geom.ctuSize - 1) / L.geom.ctuSize;
+  P.ctuLog2 = ctu_log2(L.geom); P.ctusW = (L.geom.width + L.geom.ctuSize - 1) / L.geom.ctuSize; P.ctusH = (L.geom.height + L.geom.ctuSize - 1) / L.geom.ctuSize;
   // Measurement and test switch, read on every launch (one getenv per picture): B200_INTRA_KERNEL=v1 (one CTA per block through global memory) or v2
   // (CTU-resident); unset or any other value: chosen by density.  v2 (CTU-resident) shortens the dependency chains of dense lists (I pictures); the
   // scattered intra CUs of a B picture have almost no chains and finish sooner with v1's one-CTA-per-block throughput (measured at 4K: 15 % intra CUs

@@ -23,6 +23,8 @@ __host__ __device__ inline const char* geom_problem(const b200_geom& g, int maxB
   }
   return nullptr;
 }
+// log2 of the CTU size of a geometry geom_problem accepts
+__host__ __device__ inline int ctu_log2(const b200_geom& g) { return g.ctuSize == 128 ? 7 : g.ctuSize == 64 ? 6 : 5; }
 
 // ---- K2: PU records (b200_pu) ----
 struct PuLimits { int numSlots, bitDepth, numWp, W, H; unsigned numDmvr; };
@@ -92,7 +94,6 @@ __host__ __device__ inline const char* tu_problem(const b200_tu& t, const TuLimi
 }
 
 // ---- K6: intra block records (b200_intra_tu): everything K6 uses as an address ----
-__host__ __device__ inline int intra_ctu_log2(const b200_geom& g) { return g.ctuSize == 128 ? 7 : g.ctuSize == 64 ? 6 : 5; }
 // prev = the record before t in the list (null for the first): the region before an ISP region must be the record before it
 __host__ __device__ inline const char* intra_problem(const b200_intra_tu& t, const b200_intra_tu* prev, const b200_geom& g)
 {
@@ -114,7 +115,7 @@ __host__ __device__ inline const char* intra_problem(const b200_intra_tu& t, con
   }
   // the CTU-resident kernel addresses its tile by the CTU of the block's top-left sample (chroma: CTU size halved), so a block (or ISP region) reaching
   // into the next CTU would write outside its tile rows
-  const int cl = intra_ctu_log2(g) - (t.comp ? 1 : 0);
+  const int cl = ctu_log2(g) - (t.comp ? 1 : 0);
   if ((t.x >> cl) != ((t.x + w - 1) >> cl) || (t.y >> cl) != ((t.y + h - 1) >> cl)) return "not inside one CTU";
   if (t.flags & B200_INTRA_ISP) return nullptr;
   const int pw = t.comp ? W >> 1 : W, ph = t.comp ? H >> 1 : H, unit = t.comp ? 2 : 4, m = t.multiRefIdx;
