@@ -207,6 +207,20 @@ __host__ __device__ inline const char* lmcs_vpdu_problem(const b200_lmcs_vpdu& v
   return nullptr;
 }
 
+// ---- K3: the reach of each side of one luma edge ----
+// len is the signalled length (1, 2, 3, 5 or 7).  At a CTU row (ctuRowP: a horizontal edge on a CTU's top row) the P side is never large, and beside a
+// large side a short one filters as 3.  A side writes at most `writes` samples and reads `reads`: writes + 1, and 3 for lengths 1 and 2, whose decisions
+// still read p2 / q2.  lf_kernel loads exactly these samples; lf_grid_problem spaces the edges of a line by them.
+struct LfSide { int len, writes, reads; bool large; };
+struct LfSides { LfSide p, q; };
+__host__ __device__ inline LfSides lf_sides(int sideMaxFiltLength, bool ctuRowP)
+{
+  const int lenP = (sideMaxFiltLength >> 4) & 7, lenQ = sideMaxFiltLength & 7, nP = ctuRowP && lenP > 3 ? 3 : lenP;
+  const bool large = nP > 3 || lenQ > 3;
+  const auto side = [large](int len, int n) { const int w = large && n < 3 ? 3 : n; return LfSide{len, w, w < 3 ? 3 : w + 1, n > 3}; };
+  return {side(lenP, nP), side(lenQ, lenQ)};
+}
+
 // ---- K3: the deblocking grid of one direction (dir 0: lfV, 1: lfH) ----
 // K3's flat pass (k3_deblock.cu) is exact only when no edge reads a sample that another edge of the same direction writes, and it reads no sample outside
 // the plane.  One raster scan (host only; the picture path runs the grids the glue flattens from the reference's own edge derivation unchecked); on a
@@ -214,7 +228,6 @@ __host__ __device__ inline const char* lmcs_vpdu_problem(const b200_lmcs_vpdu& v
 inline const char* lf_grid_problem(const b200_geom& g, const b200_lf_param* grid, int dir, int* x, int* y)
 {
   const int W4 = g.width >> 2, H4 = g.height >> 2, extent = dir ? g.height : g.width;
-  const auto reads = [](int n) { return n < 3 ? 3 : n + 1; };   // samples a side of effective length n reads: n + 1, and p2/q2 for the decisions of lengths 1 and 2
   const auto legal = [](int n) { return n == 1 || n == 2 || n == 3 || n == 5 || n == 7; };
   std::vector<int> prev(dir ? W4 : H4, -1), prevWQ(prev.size()), prevRQ(prev.size());   // per line: the last luma edge and its Q side's writes / reads
   for (int y4 = 0; y4 < H4; y4++)
@@ -226,16 +239,12 @@ inline const char* lf_grid_problem(const b200_geom& g, const b200_lf_param* grid
       if ((bs & 3) == 3 || ((bs >> 2) & 3) == 3 || (bs >> 4) == 3) return "Bs 3";
       if (pos == 0) return "Bs != 0 on the picture's border";
       if (!(bs & 3)) continue;                                  // chroma only: 4:2:0 chroma edges are 8 samples apart and read 4 per side
-      int nP = (e.sideMaxFiltLength >> 4) & 7;
-      const int nQ = e.sideMaxFiltLength & 7;
-      if (!legal(nP) || !legal(nQ)) return "luma filter lengths (1, 2, 3, 5 or 7)";
-      if (dir && (pos & (g.ctuSize - 1)) == 0 && nP > 3) nP = 3;   // a CTU row: the P side is never large
-      const bool large = nP > 3 || nQ > 3;                       // the long filter runs a short side as length 3
-      const int wP = large && nP < 3 ? 3 : nP, wQ = large && nQ < 3 ? 3 : nQ, rP = reads(wP), rQ = reads(wQ);
-      if (pos < rP || pos + rQ > extent) return "filter lengths read outside the picture";
-      if (prev[line] >= 0 && (pos - prev[line] < prevWQ[line] + rP || pos - prev[line] < prevRQ[line] + wP))
+      const LfSides s = lf_sides(e.sideMaxFiltLength, dir && (pos & (g.ctuSize - 1)) == 0);
+      if (!legal(s.p.len) || !legal(s.q.len)) return "luma filter lengths (1, 2, 3, 5 or 7)";
+      if (pos < s.p.reads || pos + s.q.reads > extent) return "filter lengths read outside the picture";
+      if (prev[line] >= 0 && (pos - prev[line] < prevWQ[line] + s.p.reads || pos - prev[line] < prevRQ[line] + s.p.writes))
         return "reads or writes samples the previous edge of its line writes or reads";
-      prev[line] = pos; prevWQ[line] = wQ; prevRQ[line] = rQ;
+      prev[line] = pos; prevWQ[line] = s.q.writes; prevRQ[line] = s.q.reads;
     }
   return nullptr;
 }
