@@ -28,7 +28,30 @@ constexpr int IT_ARR = IT_ORG + 2 * 64 + 80; // main / side arrays (M: the proje
 
 // one block's shared-memory scratch: reference arrays ([0] unfiltered, [1] filtered), M / S, CCLM's down-sampled luma of the block, of the row above and of
 // the column left and its (a, b, shift), DC's sum; next: intra_ctu_kernel's block tickets
-struct IntraScratch { int16_t T[2][IT_REF], L[2][IT_REF], M[IT_ARR], S[IT_ARR], Lm[32 * 32], LmTop[64], LmLeft[64]; int LmPar[4]; int next[2], sum; };
+struct IntraScratch {
+  int16_t T[2][IT_REF], L[2][IT_REF], M[IT_ARR], S[IT_ARR], Lm[32 * 32], LmTop[64], LmLeft[64]; int LmPar[4]; int next[2], sum;
+#ifdef B200_K6_PHASES
+  long long clk[5];                                          // thread 0's clock64 at the start of the block and at the end of its first four phases
+#endif
+};
+
+// Attribution build (-DB200_K6_PHASES, tools/k6_phases.py): cycles of each phase of intra_block summed over the blocks, per kernel (intra_kernel,
+// intra_ctu_kernel) and channel (luma, chroma): wait, reference fill, reference filter, prediction and store, publish, and the block count.  Thread 0 of
+// the block's threads takes the stamps; a phase that ends in a barrier includes the group's slowest thread, prediction and store end at thread 0's last
+// store, so publish includes the other threads' stores, the fence and the barrier.  The default build has none of this.
+#ifdef B200_K6_PHASES
+__device__ unsigned long long g_k6Phases[2][2][6];
+#define K6_STAMP(S, i) do { if (tid == 0) (S).clk[i] = clock64(); } while (0)
+__device__ __forceinline__ void k6_phases_add(int kernel, int comp, const long long* clk)
+{
+  const long long end = clock64();
+  unsigned long long* a = g_k6Phases[kernel][comp ? 1 : 0];
+  for (int i = 0; i < 4; i++) atomicAdd(a + i, (unsigned long long)(clk[i + 1] - clk[i]));
+  atomicAdd(a + 4, (unsigned long long)(end - clk[4])); atomicAdd(a + 5, 1ull);
+}
+#else
+#define K6_STAMP(S, i) do {} while (0)
+#endif
 
 __constant__ int cAng[32] = {0, 1, 2, 3, 4, 6, 8, 10, 12, 14, 16, 18, 20, 23, 26, 29, 32, 35, 39, 45, 51, 57, 64, 73, 86, 102, 128, 171, 256, 341, 512, 1024};
 __constant__ int cInvAng[32] = {0, 16384, 8192, 5461, 4096, 2731, 2048, 1638, 1365, 1170, 1024, 910, 819, 712, 630, 565,
@@ -129,7 +152,24 @@ __device__ __forceinline__ void intra_block(const IntraParams& P, const b200_int
   const int availTL = (t.flags & B200_INTRA_AVAIL_TL) ? 1 : 0, numAbove = t.numAbove, numLeft = t.numLeft;
   const IspGeom g(t);
   const int bx = g.bx, by = g.by;
+  K6_STAMP(S, 0);
   if (tid == 0) S.sum = 0;
+  // what reads no neighbour sample comes before the wait, which it then overlaps: the reference extents, where results go, the angular parameters
+  // (bx, by, bw, bh): the block the neighbourhood was analysed for — the block itself, or the CU of an ISP region
+  const int topLen = g.topLen, sideLen = g.sideLen, predSize = 2 * g.bw, predHSize = 2 * g.bh;
+  const int totalUnits = (predSize + unit - 1) / unit + (predHSize + unit - 1) / unit + 1, n = availTL + numAbove + numLeft;
+  const int aboveLen = min(numAbove * unit, predSize), leftLen = min(numLeft * unit, predHSize);
+  const int mode = t.mode;
+  const bool doPDPC = w >= 4 && h >= 4 && mrl == 0;
+  // results go where `io` puts them; the CIIP inter prediction and the residual are read from the same place
+  int16_t* dst = io.out(x0, y0);
+  const int dp = io.pitch();
+  const int16_t* rs = (P.resi[c] && (t.flags & B200_INTRA_ADD_RESI)) ? io.resi(x0, y0) : nullptr;
+  const int ciipW = g.isp ? 0 : t.ciip;                      // CIIP: the block holds the inter prediction; blend (predBlendIntraCiip :925-938)
+  const int predMode = wide_angle(g.bw, g.bh, mode);         // angular modes; ISP: the CU decides (:610)
+  const bool ver = predMode >= 34;
+  const int angMode = ver ? predMode - 50 : -(predMode - 18), absMode = abs(angMode);    // < 32 for every mode
+  const int invAngle = cInvAng[absMode], absAng = cAng[absMode];
 
   // ---- wait for the earlier blocks this one reads from
   if (g.k && tid == 0) io.wait(me - 1);                                // ISP: the region before this one is the record before it
@@ -150,12 +190,9 @@ __device__ __forceinline__ void intra_block(const IntraParams& P, const b200_int
     for (int u = tid; u < nU; u += IT_THREADS) { const int o = io.owner(0, ux0 + u % uw, uy0 + u / uw); if (o >= 0 && o < me) io.wait(o); }
   }
   intra_sync(bar);
+  K6_STAMP(S, 1);
 
   // ---- reference samples (xFillReferenceSamples): T[j] = row above incl. the corner, L[i] = left column, T[0] = L[0] = corner
-  // (bx, by, bw, bh): the block the neighbourhood was analysed for — the block itself, or the CU of an ISP region
-  const int topLen = g.topLen, sideLen = g.sideLen, predSize = 2 * g.bw, predHSize = 2 * g.bh;
-  const int totalUnits = (predSize + unit - 1) / unit + (predHSize + unit - 1) / unit + 1, n = availTL + numAbove + numLeft;
-  const int aboveLen = min(numAbove * unit, predSize), leftLen = min(numLeft * unit, predHSize);
   auto pix = [&](int x, int y) -> int { return io.pix(c, x, y); };
   auto refT = [&](int j) -> int {                              // row above (bx, by) incl. the corner: xFillReferenceSamples :1072
     if (n == 0) return 1 << (P.bitDepth - 1);
@@ -206,6 +243,7 @@ __device__ __forceinline__ void intra_block(const IntraParams& P, const b200_int
     }
   }
   intra_sync(bar);
+  K6_STAMP(S, 2);
   if ((t.flags & B200_INTRA_FILTER_REF) && !c && !mrl) {     // xFilterReferenceSamples
     int16_t *FT = S.T[1], *FL = S.L[1];
     for (int j = tid; j <= predSize; j += IT_THREADS)
@@ -217,14 +255,8 @@ __device__ __forceinline__ void intra_block(const IntraParams& P, const b200_int
     T = FT; L = FL;
     intra_sync(bar);
   }
+  K6_STAMP(S, 3);
 
-  const int mode = t.mode;
-  const bool doPDPC = w >= 4 && h >= 4 && mrl == 0;
-  // results go where `io` puts them; the CIIP inter prediction and the residual are read from the same place
-  int16_t* dst = io.out(x0, y0);
-  const int dp = io.pitch();
-  const int16_t* rs = (P.resi[c] && (t.flags & B200_INTRA_ADD_RESI)) ? io.resi(x0, y0) : nullptr;
-  const int ciipW = g.isp ? 0 : t.ciip;                      // CIIP: the block holds the inter prediction; blend (predBlendIntraCiip :925-938)
   auto store = [&](int x, int y, int v) {
     int16_t* d = dst + y * dp + x;
     if (ciipW) v = ((4 - ciipW) * (int)*d + ciipW * v + 2) >> 2;
@@ -380,10 +412,7 @@ __device__ __forceinline__ void intra_block(const IntraParams& P, const b200_int
     for (int k = tid; k < w * h; k += IT_THREADS) { const int y = k >> t.log2w, x = k & (w - 1); store(x, y, mode == B200_INTRA_BDPCM_HOR ? L[y + 1] : T[x + 1]); }
   } else {
     // ---- angular (xPredIntraAng): every sample on its own from the main / side references
-    const int predMode = wide_angle(g.bw, g.bh, mode);             // ISP: the CU decides (:610)
-    const bool ver = predMode >= 34;
-    const int angMode = ver ? predMode - 50 : -(predMode - 18), absMode = abs(angMode);
-    const int invAngle = cInvAng[absMode], absAng = cAng[absMode], angle = angMode < 0 ? -absAng : absAng;
+    const int angle = angMode < 0 ? -absAng : absAng;
     const int16_t *mainSrc = ver ? T : L, *sideSrc = ver ? L : T;
     const int mw = ver ? w : h, mh = ver ? h : w;            // block size along the main / the side reference
     // angles >= 0 read the main reference directly, clamped to its end (the replication tail of xPredIntraAng); negative angles stage the main array
@@ -433,6 +462,7 @@ __device__ __forceinline__ void intra_block(const IntraParams& P, const b200_int
       if (ver) store(xx, yy, v); else store(yy, xx, v);
     }
   }
+  K6_STAMP(S, 4);
 }
 
 // intra_kernel: samples, owner words and done words in global memory; a block's results go to the plane
@@ -472,6 +502,9 @@ __global__ void __launch_bounds__(IT_THREADS, 12) intra_kernel(const IntraParams
     __threadfence();
     __syncthreads();
     if (tid == 0) atomicExch(P.done + me, 1);
+#ifdef B200_K6_PHASES
+    if (tid == 0) k6_phases_add(0, t.comp, S.clk);
+#endif
   }
 }
 
@@ -549,7 +582,8 @@ struct TileIo {
   {
     int spins = 0;
     if (o >= first) {
-      while (sflag[o - first] == 0) { if (++spins > 64) __nanosleep(20); if (spins > (1 << 24)) { atomicOr(P.err, 1); break; } }
+      // every re-poll sleeps 20 ns: the 4K I picture's K6 is 0.8 % faster than with 64 tight spins first, and slower with 100 or 300 ns (H100, 700 W)
+      while (sflag[o - first] == 0) { __nanosleep(20); if (++spins > (1 << 24)) { atomicOr(P.err, 1); break; } }
       __threadfence_block();
       return;
     }
@@ -635,6 +669,9 @@ __global__ void __launch_bounds__(V2_THREADS, 1) intra_ctu_kernel(const IntraPar
         __threadfence_block();
         sflag[k] = 1;
         if (t.x + (1 << t.log2w) == (cx >> s) + (cw >> s) || t.y + (1 << t.log2h) == (cy >> s) + (ch >> s)) v2_st_release(P.done + me, 1);
+#ifdef B200_K6_PHASES
+        k6_phases_add(1, t.comp, S.clk);
+#endif
       }
     }
   }
@@ -765,3 +802,13 @@ int launch_intra(const IntraLaunch& L, cudaStream_t s, KHook* hook)
 }
 
 }  // namespace b200
+
+#ifdef B200_K6_PHASES
+// the attribution build's counters: copies them to out[2][2][6] (see g_k6Phases) after the device is idle, and clears them if `reset`
+extern "C" B200_API int b200_k6_phases(unsigned long long* out, int reset)
+{
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, b200::g_k6Phases, sizeof(b200::g_k6Phases)) != cudaSuccess) return -1;
+  if (reset) { static const unsigned long long zero[2][2][6] = {}; if (cudaMemcpyToSymbol(b200::g_k6Phases, zero, sizeof(zero)) != cudaSuccess) return -1; }
+  return 0;
+}
+#endif
