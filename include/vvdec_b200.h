@@ -105,7 +105,8 @@ B200_API int b200_k1_residual(const b200_geom* g, int16_t* const planes[3],
  *             xEdgeFilterChroma (:1619), LoopFilter::xPelFilterLuma (LoopFilter.h:106; xPelFilterLumaCore :213),
  *             LoopFilter::xFilteringPandQ (LoopFilter.h:122; xFilteringPandQCore :129), xPelFilterChroma (:281),
  *             xUseStrongFiltering (:1410), xCalcDP/DQ (:1392), deriveLADFShift (:1363).
- *   stays CPU: calcFilterStrengthsCTU (:360) — it produces the grid below from the CU/TU tree (SURVEY a14').
+ *   stays CPU: calcFilterStrengthsCTU (:360) — it produces the grid below from the CU/TU tree (SURVEY a14'), unless the picture asks the device
+ *             to derive the grids from CU / TU records (B200_PIC_DERIVE_LF, b200_lf_derive below).
  * The edge grids are the reference's LoopFilterParam arrays (TypeDef.h:694, DecLibRecon.cpp:515) re-laid as one
  * picture-wide raster per direction: entry (x4,y4) describes the edge on the LEFT (lfV) / TOP (lfH) of the 4x4
  * luma unit at (4*x4, 4*y4).  Chroma uses the same entries on its 8x8-sample grid (LoopFilter.cpp:462-488).
@@ -145,6 +146,55 @@ typedef struct b200_lf_seq {        /* SPS luma-adaptive deblocking (LADF), Slic
  * calcFilterStrengths derives, as the glue flattens them, are legal. */
 B200_API int b200_lf_deblock(const b200_geom* g, int16_t* const planes[3], const b200_lf_param* lfV, const b200_lf_param* lfH,
                              const uint8_t* ctuSlice, const b200_lf_slice* slices, int numSlices, const b200_lf_seq* seq, int dirs);
+
+/* Edge grids derived on the device (B200_PIC_DERIVE_LF): the picture carries its coding units and transform units instead of lfV / lfH, and
+ * b200_pic_run derives both grids before K3 — LoopFilter::calcFilterStrengthsCTU (LoopFilter.cpp:360) with calcFilterStrengths (:495),
+ * xSetMaxFilterLengthPQFromTransformSizes (:780), xSetMaxFilterLengthPQForCodingSubBlocks (:707), xSetEdgeFilterInsidePu (:1032) and
+ * xGetBoundaryStrengthSingle (:1094), from a 4x4 motion field built out of the picture's b200_pu records (what MIDER stores, before the DMVR
+ * deltas).  The grids are byte-identical to what the glue's flattenLfCtu copies out of the reference's per-CTU arrays.  IBC and virtual
+ * boundaries are not part of it (the glue refuses both).
+ * One b200_lf_cu per coding unit, in the order cs.traverseCUs walks each CTU, CTUs in raster order (b200_picture::lfCtuCus holds where each CTU's
+ * CUs start); one b200_lf_tu per transform unit of a CU, coefficients or not, in the CU's TU order. */
+enum {
+  B200_LF_CU_INTRA = 1,       /* predMode MODE_INTRA (else MODE_INTER)                                                */
+  B200_LF_CU_CIIP = 2, B200_LF_CU_AFFINE = 4, B200_LF_CU_SBTMVP = 8 /* merge type MRG_TYPE_SUBPU_ATMVP */, B200_LF_CU_GEO = 16,
+  B200_LF_CU_ISP = 32,        /* ispMode() != 0                                                                        */
+  B200_LF_CU_BDPCM_Y = 64, B200_LF_CU_BDPCM_C = 128,   /* bdpcmMode() / bdpcmModeChroma() != 0                          */
+  B200_LF_CU_AVAIL_LEFT = 256, B200_LF_CU_AVAIL_TOP = 512,   /* xGetLoopfilterParam (:1063): leftEdge / topEdge            */
+  B200_LF_CU_SEP_TREE = 1024  /* CU::isSepTree: the CU covers one channel type only                                    */
+};
+typedef struct b200_lf_cu {
+  uint16_t x, y;              /* cu.blocks[chType]: position and size in samples of its channel type                  */
+  uint8_t  w, h;
+  uint8_t  chType;            /* 0 luma (with chroma unless B200_LF_CU_SEP_TREE), 1 chroma                             */
+  uint8_t  treeType;          /* cu.treeType(): 0 TREE_D, 1 TREE_L, 2 TREE_C                                           */
+  uint16_t flags;             /* B200_LF_CU_*                                                                          */
+  int8_t   qp;                /* cu.qp                                                                                 */
+  uint8_t  slice;             /* index into b200_picture::lfSlices / lfSliceB                                          */
+  uint8_t  geoLists;          /* GEO: bit p = partition p predicts from list 1 (interDirrefIdxGeo0 / 1)                */
+  uint8_t  numTus;            /* transform units of the CU: lfTus[firstTu .. firstTu + numTus - 1]                    */
+  uint8_t  rsv[2];
+  uint32_t firstTu;
+  uint32_t firstPu;           /* inter CUs: its first b200_pu record (SbTMVP runs follow it); intra CUs: unused      */
+} b200_lf_cu;                 /* 24 bytes */
+typedef struct b200_lf_tu {
+  uint16_t x, y; uint8_t w, h;        /* tu.blocks[Y] as the reference holds it (w = h = 0: no luma block)          */
+  uint16_t cx, cy; uint8_t cw, ch;    /* tu.blocks[Cb] in chroma samples (cw = ch = 0: no chroma block)             */
+  uint8_t  cbf;                       /* tu.cbf: bit c = coded block flag of component c                             */
+  uint8_t  jointCbCr;
+  int8_t   chromaQp[2];               /* tu.chromaQp (LoopFilter.cpp:1127-1128)                                      */
+} b200_lf_tu;                         /* 16 bytes */
+/* Kernel-level edge derivation: the lfV / lfH rasters ([H/4][W/4], host memory) of the records, derived on the device as b200_pic_run does for
+ * B200_PIC_DERIVE_LF.  ctuCus: [number of CTUs + 1] as b200_picture::lfCtuCus; pus: the picture's b200_pu records (the motion field); slices / sliceB:
+ * numSlices entries as b200_picture::lfSlices / lfSliceB.  Returns B200_ERR_PARAM, before any device work and with lfV / lfH untouched, for an invalid
+ * geometry (b200_geom), numSlices outside 1..64, CTU ranges that do not run from 0 to numCus without going back, and a record the picture path refuses
+ * too: a CU whose block (in its channel type) or one of whose TU blocks lies outside its plane or outside the CTU whose range lists the CU, an undefined
+ * channel, tree type or flag, a slice index >= numSlices, no TU or TU records past numTus.  Records that pass but do not tile the picture the way a
+ * coding tree does give undefined grids. */
+struct b200_pu;
+B200_API int b200_lf_derive(const b200_geom* g, const b200_lf_cu* cus, size_t numCus, const b200_lf_tu* tus, size_t numTus, const uint32_t* ctuCus,
+                            const struct b200_pu* pus, size_t numPus, const b200_lf_slice* slices, const uint8_t* sliceB, int numSlices,
+                            b200_lf_param* lfV, b200_lf_param* lfH);
 
 /* ------------------------------------------------------------------------------------------------
  * K4  SAO: src (deblocked picture) -> dst, per CTU and component edge offset (4 directions) or band offset.
@@ -404,8 +454,13 @@ typedef struct b200_picture {
   const b200_intra_tu* intraTus;         /* K6: intra blocks of the picture in decoding order, or NULL.  Runs after K2 and K1: blocks read the     */
   size_t numIntraTus;                    /* reconstruction of inter and earlier intra neighbours.  With LMCS chroma scaling: luma blocks, then the
                                             per-VPDU scales, then the chroma blocks (see "with LMCS" above)                                     */
+  /* B200_PIC_DERIVE_LF (with B200_PIC_DEBLOCK; lfV and lfH must then be NULL): the records the device derives both grids from (see b200_lf_cu) */
+  const b200_lf_cu* lfCus; size_t numLfCus;
+  const b200_lf_tu* lfTus; size_t numLfTus;
+  const uint32_t* lfCtuCus;              /* [number of CTUs + 1]: index of each CTU's first CU record (raster order), then numLfCus            */
+  const uint8_t* lfSliceB;               /* [numLfSlices]: 1 for a B slice (Slice::isInterB, LoopFilter.cpp:1235)                          */
 } b200_picture;
-enum { B200_PIC_DEBLOCK = 1, B200_PIC_SAO = 2, B200_PIC_ALF = 4, B200_PIC_LMCS = 8 };
+enum { B200_PIC_DEBLOCK = 1, B200_PIC_SAO = 2, B200_PIC_ALF = 4, B200_PIC_LMCS = 8, B200_PIC_DERIVE_LF = 16 };
 
 /* create(): reference DecLibRecon::create (DecLibRecon.cpp:392). numSlots = DPB size, numArenas = pictures whose work
  * lists may be resident at once (>= 2 for upload/compute overlap). device < 0: current device.  Returns B200_ERR_PARAM for an
@@ -493,7 +548,8 @@ B200_API long long b200_ctx_kernel_launches(b200_ctx* ctx);
  * Families: 0 K2 translational tiles, 1 K2 affine tiles, 2 K1, 3 K3 vertical, 4 K3 horizontal, 5 K4, 6 K5 luma, 7 K5 chroma.
  * set_profiling(1) enables event recording (adds a few us per picture); get_kernel_ms sums and resets the collected times. */
 enum { B200_KF_MC_TILE = 0, B200_KF_MC_AFFINE, B200_KF_K1, B200_KF_LF_V, B200_KF_LF_H, B200_KF_SAO, B200_KF_ALF_LUMA, B200_KF_ALF_CHROMA,
-       B200_KF_INTRA /* K6 incl. its ordering pre-passes */, B200_KF_LMCS /* per-VPDU scale + inverse map */, B200_KF_COUNT };
+       B200_KF_INTRA /* K6 incl. its ordering pre-passes */, B200_KF_LMCS /* per-VPDU scale + inverse map */,
+       B200_KF_LF_DERIVE /* B200_PIC_DERIVE_LF: CU maps, motion field, edge grids */, B200_KF_COUNT };
 B200_API int  b200_ctx_set_profiling(b200_ctx* ctx, int on);
 B200_API int  b200_ctx_get_kernel_ms(b200_ctx* ctx, float ms[8], int counts[8]);          /* the first eight families */
 B200_API int  b200_ctx_get_kernel_ms_n(b200_ctx* ctx, float* ms, int* counts, int n);     /* n <= B200_KF_COUNT families */

@@ -156,8 +156,30 @@ def lmcs():
     np.savez_compressed(os.path.join(OUT, "lmcs_pictures.npz"), **out)
 
 
+LF_DERIVE_CASES = [("B_mixed", 1, (416, 240)), ("B_affine_heavy", 2, (416, 240)), ("I_picture", 1, (416, 240)), ("P_picture", 2, (416, 240)), ("B_isp", 3, (416, 240)),
+                   ("B_5slices_no_lf_across_ctu64", 1, (416, 240)), ("I_6slices_no_lf_across_ctu64", 2, (416, 240)), ("B_local_dual_tree_isp", 1, (416, 240)),
+                   ("I_local_dual_tree", 3, (416, 240)), ("B_ctu32_8bit", 1, (200, 136)), ("B_mixed", 2, (200, 136)), ("B_3slices", 3, (416, 240))]
+
+
+def lf_derive():
+    """Seam pictures (tests/test_lf_derive_cpu.py CASES) as the drop-in class flattens them with the device edge derivation switched on — CU / TU / PU records,
+    CTU ranges, slice tables — and the reference's own edge grids of the same pictures (calcFilterStrengthsCTU + flattenLfCtu)."""
+    from tests.test_lf_derive_cpu import CASES, flatten_grids, records_of
+    out = dict(names=np.array([f"{n}-s{s}-{w}x{h}" for n, s, (w, h) in LF_DERIVE_CASES]))
+    for k, (name, seed, (w, h)) in enumerate(LF_DERIVE_CASES):
+        case = helpers.SeamCase(ref, np.random.default_rng(seed), w, h, **CASES[name])
+        wantV, wantH, _ = flatten_grids(case, False)
+        _, _, flat = flatten_grids(case, True)
+        r = records_of(flat, case.g)
+        g = case.g
+        out[f"{k}_geom"] = np.array([g.width, g.height, g.chromaFormat, g.bitDepth, g.ctuSize], np.int32)
+        out.update({f"{k}_{f}": v for f, v in r.items()})
+        out[f"{k}_lfV"] = wantV; out[f"{k}_lfH"] = wantH
+    np.savez_compressed(os.path.join(OUT, "lf_derive_pictures.npz"), **out)
+
+
 if __name__ == "__main__":
     import sys
     if len(sys.argv) > 1: [globals()[n]() for n in sys.argv[1:]]
-    else: k1(); pictures(); chain(); film_grain(); intra(); lmcs()
+    else: k1(); pictures(); chain(); film_grain(); intra(); lmcs(); lf_derive()
     print({f: os.path.getsize(os.path.join(OUT, f)) for f in sorted(os.listdir(OUT))})

@@ -73,7 +73,17 @@ def const_plane_ptrs(planes):
     return plane_ptrs(planes)
 
 
-PIC_DEBLOCK, PIC_SAO, PIC_ALF, PIC_LMCS = 1, 2, 4, 8
+PIC_DEBLOCK, PIC_SAO, PIC_ALF, PIC_LMCS, PIC_DERIVE_LF = 1, 2, 4, 8, 16
+
+# B200_PIC_DERIVE_LF records (b200_lf_cu, b200_lf_tu)
+LF_CU_INTRA, LF_CU_CIIP, LF_CU_AFFINE, LF_CU_SBTMVP, LF_CU_GEO, LF_CU_ISP, LF_CU_BDPCM_Y, LF_CU_BDPCM_C, LF_CU_AVAIL_LEFT, LF_CU_AVAIL_TOP, LF_CU_SEP_TREE = \
+    1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1024
+LF_CU_DTYPE = np.dtype([("x", "<u2"), ("y", "<u2"), ("w", "u1"), ("h", "u1"), ("chType", "u1"), ("treeType", "u1"), ("flags", "<u2"), ("qp", "i1"),
+                        ("slice", "u1"), ("geoLists", "u1"), ("numTus", "u1"), ("rsv", "u1", (2,)), ("firstTu", "<u4"), ("firstPu", "<u4")])
+LF_TU_DTYPE = np.dtype([("x", "<u2"), ("y", "<u2"), ("w", "u1"), ("h", "u1"), ("cx", "<u2"), ("cy", "<u2"), ("cw", "u1"), ("ch", "u1"),
+                        ("cbf", "u1"), ("jointCbCr", "u1"), ("chromaQp", "i1", (2,))])
+assert LF_CU_DTYPE.itemsize == 24 and LF_TU_DTYPE.itemsize == 16
+LF_PARAM_DTYPE = np.dtype([("qp", "i1", (3,)), ("bs", "u1"), ("sideMaxFiltLength", "u1"), ("flags", "u1")])
 
 
 class Picture(C.Structure):
@@ -84,7 +94,9 @@ class Picture(C.Structure):
                 ("lfV", C.c_void_p), ("lfH", C.c_void_p), ("ctuSlice", C.c_void_p), ("lfSlices", C.c_void_p),
                 ("numLfSlices", C.c_int32), ("lfSeq", C.c_void_p),
                 ("sao", C.c_void_p), ("vb", C.c_void_p), ("alf", C.c_void_p), ("alfTabs", C.c_void_p), ("wp", C.c_void_p), ("numWp", C.c_int32), ("lmcs", C.c_void_p),
-                ("intraTus", C.c_void_p), ("numIntraTus", C.c_size_t)]
+                ("intraTus", C.c_void_p), ("numIntraTus", C.c_size_t),
+                ("lfCus", C.c_void_p), ("numLfCus", C.c_size_t), ("lfTus", C.c_void_p), ("numLfTus", C.c_size_t),
+                ("lfCtuCus", C.c_void_p), ("lfSliceB", C.c_void_p)]
 
 
 class LmcsVpdu(C.Structure):

@@ -19,6 +19,9 @@ def declare(lib):
     lib.b200_lf_deblock.argtypes = [C.POINTER(abi.Geom), PLANES, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                     C.c_void_p, C.c_int]
     lib.b200_lf_deblock.restype = C.c_int
+    lib.b200_lf_derive.argtypes = [C.POINTER(abi.Geom), C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
+                                   C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.b200_lf_derive.restype = C.c_int
 
 
     lib.b200_sao_picture.argtypes = [C.POINTER(abi.Geom), PLANES, PLANES, C.c_void_p, C.c_void_p]
@@ -65,5 +68,5 @@ def declare(lib):
 
 EXPORTS = ["b200_ctx_create", "b200_ctx_destroy", "b200_ctx_load_slot", "b200_decompress_picture", "b200_pic_upload", "b200_pic_run",
            "b200_wait_picture", "b200_get_frame", "b200_ctx_load_slot_strided", "b200_get_frame_strided", "b200_get_frame_async", "b200_get_frame_device_async", "b200_frame_wait", "b200_frame_bytes", "b200_get_frame_fmt_async", "b200_frame_hash_async", "b200_intra_predict", "b200_intra_reconstruct", "b200_get_frame_grain_async", "b200_ctx_mark", "b200_ctx_elapsed_ms", "b200_ctx_kernel_launches", "b200_ctx_set_profiling", "b200_ctx_get_kernel_ms", "b200_ctx_get_kernel_ms_n", "b200_host_register", "b200_host_unregister",
-           "b200_mc_predict", "b200_mc_predict_wp", "b200_last_error", "b200_version", "b200_device_count", "b200_k1_residual", "b200_lf_deblock",
+           "b200_mc_predict", "b200_mc_predict_wp", "b200_last_error", "b200_version", "b200_device_count", "b200_k1_residual", "b200_lf_deblock", "b200_lf_derive",
            "b200_sao_picture", "b200_alf_picture"]

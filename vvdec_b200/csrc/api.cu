@@ -1,6 +1,7 @@
 // api.cu — C-ABI entry points of libvvdec_b200.so (include/vvdec_b200.h). Host-pointer wrappers stage
 // through device scratch buffers; picture-level entry points keep everything resident (see picture.cu).
 #include "common.cuh"
+#include "lf_derive.cuh"
 #include <stdarg.h>
 #include <string.h>
 #include <mutex>
@@ -143,6 +144,41 @@ B200_API int b200_lf_deblock(const b200_geom* g, int16_t* const planes[3], const
   if (int rc = st.commit(g_hw.buf, s)) return rc;
   if (int rc = launch_lf_deblock(L, s)) return rc;
   if (int rc = download_planes(g, planes, L.planes, s)) return rc;
+  B200_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+B200_API int b200_lf_derive(const b200_geom* g, const b200_lf_cu* cus, size_t numCus, const b200_lf_tu* tus, size_t numTus, const uint32_t* ctuCus,
+                            const b200_pu* pus, size_t numPus, const b200_lf_slice* slices, const uint8_t* sliceB, int numSlices, b200_lf_param* lfV, b200_lf_param* lfH)
+{
+  const char* fn = "b200_lf_derive";
+  B200_CHECK(g && cus && numCus && tus && ctuCus && (pus || !numPus) && slices && sliceB && lfV && lfH, "b200_lf_derive: null argument");
+  B200_CHECK(numSlices >= 1 && numSlices <= 64, "b200_lf_derive: numSlices %d out of range 1..64", numSlices);
+  if (!rule_ok(fn, geom_problem(*g, 12, 1))) return B200_ERR_PARAM;
+  const size_t n4 = (size_t)(g->width >> 2) * (g->height >> 2);
+  const int nCtu = ((g->width + g->ctuSize - 1) / g->ctuSize) * ((g->height + g->ctuSize - 1) / g->ctuSize);
+  B200_CHECK(ctuCus[0] == 0 && ctuCus[nCtu] == numCus, "b200_lf_derive: the CTU ranges do not cover the CU records from 0 to numCus");
+  const LfLimits lim = lf_limits(*g, numSlices, numTus);
+  for (int a = 0; a < nCtu; a++) {
+    B200_CHECK(ctuCus[a] <= ctuCus[a + 1], "b200_lf_derive: the CU range of CTU %d ends before it starts", a);
+    for (uint32_t i = ctuCus[a]; i < ctuCus[a + 1]; i++)
+      if (const char* why = lf_cu_problem(cus[i], tus, a, lim)) { set_error("b200_lf_derive: CU record %u of CTU %d: %s", i, a, why); return B200_ERR_PARAM; }
+  }
+  if (int rc = ensure_device()) return rc;
+  if (int rc = g_hw.init()) return rc;
+  cudaStream_t s = g_hw.stream;
+  LfDeriveLaunch L{}; L.geom = *g; L.numCus = numCus; L.numPus = numPus;
+  Staging st;
+  st.add(&L.cus, cus, numCus); st.add(&L.tus, tus, numTus); st.add(&L.ctuCus, ctuCus, (size_t)nCtu + 1); st.add(&L.pus, pus, numPus);
+  st.add(&L.slices, slices, (size_t)numSlices); st.add(&L.sliceB, sliceB, (size_t)numSlices);
+  st.add(&L.map[0], nullptr, 2 * n4); st.add(&L.mi, nullptr, n4); st.add(&L.lfV, nullptr, n4); st.add(&L.lfH, nullptr, n4);
+  if (int rc = st.commit(g_hw.buf, s)) return rc;
+  L.map[1] = L.map[0] + n4;
+  L.anyDisabled = false;
+  for (int k = 0; k < numSlices; k++) L.anyDisabled = L.anyDisabled || slices[k].disable;
+  if (int rc = launch_lf_derive(L, s, nullptr)) return rc;
+  if (int rc = copy_host(lfV, L.lfV, n4 * sizeof(b200_lf_param), cudaMemcpyDeviceToHost, s)) return rc;
+  if (int rc = copy_host(lfH, L.lfH, n4 * sizeof(b200_lf_param), cudaMemcpyDeviceToHost, s)) return rc;
   B200_CUDA(cudaStreamSynchronize(s));
   return 0;
 }

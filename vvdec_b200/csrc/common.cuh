@@ -213,6 +213,19 @@ struct LfLaunch {
 };
 int launch_lf_deblock(const LfLaunch& L, cudaStream_t s, KHook* hook = nullptr);
 
+// B200_PIC_DERIVE_LF (lf_derive.cu): the edge grids lfV / lfH from CU / TU records; map[2] and mi are [H/4][W/4] scratch (CU maps, LfMi motion field)
+struct LfMi;
+struct LfDeriveLaunch {
+  b200_geom geom;
+  const b200_lf_cu* cus; size_t numCus; const b200_lf_tu* tus; const uint32_t* ctuCus; const b200_pu* pus; size_t numPus;
+  const b200_lf_slice* slices; const uint8_t* sliceB;
+  uint32_t* map[2]; LfMi* mi; b200_lf_param *lfV, *lfH;
+  bool anyDisabled;                 // some slice has deblocking disabled
+};
+constexpr int LM_ERR_LF_RECORD = 32;   // error bit of the PU meta block: a CU / TU record of B200_PIC_DERIVE_LF (lf_cu_problem)
+int launch_lf_validate(const b200_lf_cu* cus, size_t numCus, const b200_lf_tu* tus, size_t numTus, const uint32_t* ctuCus, const b200_geom& g, int numSlices, int* meta, cudaStream_t s, KHook* hook);
+int launch_lf_derive(const LfDeriveLaunch& L, cudaStream_t s, KHook* hook);
+
 struct SaoLaunch { b200_geom geom; DevPlanes src, dst; const b200_sao_ctu* ctus; b200_vb vb; };
 int launch_sao(const SaoLaunch& L, cudaStream_t s, KHook* hook = nullptr);
 

@@ -1,6 +1,7 @@
 // picture.cu — picture-level context: device-resident DPB, work-list arenas, and the per-picture kernel chain
 // (the device replacement of DecLibRecon::decompressPicture's CTU task graph, reference DecoderLib/DecLibRecon.cpp:429-682).
 #include "common.cuh"
+#include "lf_derive.cuh"
 #include <string.h>
 #include <vector>
 
@@ -10,7 +11,7 @@ struct Arena {
   DevBuf buf;                       // one allocation, sub-allocated per picture
   // The launch records of the picture's kernels, filled by b200_pic_upload.  b200_pic_run adds what is known at run time: planes, reference slots,
   // list counts (hMeta) and compSel.
-  McLaunch mc; K1Launch k1; IntraLaunch intra; LmcsLaunch lm; LfLaunch lf; SaoLaunch sao; AlfLaunch alf;
+  McLaunch mc; K1Launch k1; IntraLaunch intra; LmcsLaunch lm; LfLaunch lf; SaoLaunch sao; AlfLaunch alf; LfDeriveLaunch lfd;
   int* hMeta = nullptr;             // pinned host copy of both meta blocks (list lengths + error bits), valid once `uploaded` has fired
   size_t numPus = 0, numDmvr = 0;
   DevPlanes given;                  // pre-reconstructed samples, or null planes
@@ -193,7 +194,10 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
 {
   B200_CHECK(c && p, "b200_pic_upload: null argument");
   B200_CHECK(p->dstSlot >= 0 && p->dstSlot < c->numSlots, "b200_pic_upload: dstSlot %d", p->dstSlot);
-  B200_CHECK(!(p->flags & B200_PIC_DEBLOCK) || (p->lfV && p->lfH && p->lfSlices && p->numLfSlices >= 1 && p->numLfSlices <= 64), "b200_pic_upload: deblocking data missing");
+  const bool lfd = p->flags & B200_PIC_DERIVE_LF;
+  B200_CHECK(!lfd || ((p->flags & B200_PIC_DEBLOCK) && !p->lfV && !p->lfH && p->lfCus && p->numLfCus && p->lfTus && p->lfCtuCus && p->lfSliceB && p->numLfCus < (1u << 31) && p->numLfTus < (1u << 31)),
+             "b200_pic_upload: B200_PIC_DERIVE_LF needs B200_PIC_DEBLOCK, CU / TU records, CTU ranges and slice types, and no lfV / lfH");
+  B200_CHECK(!(p->flags & B200_PIC_DEBLOCK) || ((lfd || (p->lfV && p->lfH)) && p->lfSlices && p->numLfSlices >= 1 && p->numLfSlices <= 64), "b200_pic_upload: deblocking data missing");
   B200_CHECK(!(p->flags & B200_PIC_SAO) || p->sao, "b200_pic_upload: SAO data missing");
   B200_CHECK(!(p->flags & B200_PIC_ALF) || (p->alf && p->alfTabs), "b200_pic_upload: ALF data missing");
   // the O(1) rules of b200_sao_picture / b200_alf_picture (rules.cuh); the CTU records are checked on the device
@@ -225,7 +229,13 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   Staging st;
   st.add(&A.mc.pus, p->pus, p->numPus); st.add(&tiles, nullptr, capTiles); st.add(&meta, nullptr, 2 * LM_INTS); st.add(&tuIdx, nullptr, p->numTus);
   st.add(&A.k1.tus, p->tus, p->numTus); st.add(&A.k1.coefs, p->coefs, p->numCoefs); st.add(&A.k1.scaling, p->scaling, p->numScaling);
-  st.add(&A.lf.lfV, p->lfV, lf ? n4 : 0); st.add(&A.lf.lfH, p->lfH, lf ? n4 : 0); st.add(&A.lf.ctuSlice, lf ? p->ctuSlice : nullptr, nCtu);
+  st.add(&A.lf.lfV, lfd ? nullptr : p->lfV, lf ? n4 : 0); st.add(&A.lf.lfH, lfd ? nullptr : p->lfH, lf ? n4 : 0);
+  if (lfd) {                                                          // (the arena of a picture without it keeps its layout)
+    st.add(&A.lfd.cus, p->lfCus, p->numLfCus); st.add(&A.lfd.tus, p->lfTus, p->numLfTus); st.add(&A.lfd.ctuCus, p->lfCtuCus, nCtu + 1);
+    st.add(&A.lfd.sliceB, p->lfSliceB, (size_t)p->numLfSlices); st.add(&A.lfd.slices, p->lfSlices, (size_t)p->numLfSlices);
+    st.add(&A.lfd.map[0], nullptr, 2 * n4); st.add(&A.lfd.mi, nullptr, n4);
+  }
+  st.add(&A.lf.ctuSlice, lf ? p->ctuSlice : nullptr, nCtu);
   st.add(&A.sao.ctus, p->sao, sao ? nCtu : 0);
   st.add(&A.alf.ctus, p->alf, alf ? nCtu : 0); stage_alf_tables(st, A.alf, alf ? p->alfTabs : nullptr);
   st.add(&A.mc.dmvrMv, nullptr, p->numDmvr * 2);
@@ -243,6 +253,12 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   if (!lf || !p->ctuSlice) A.lf.ctuSlice = nullptr;                   // the entry is there either way, uploaded only for deblocking
   if (p->numDmvr) B200_CUDA(cudaMemsetAsync(A.mc.dmvrMv, 0, p->numDmvr * 8, s));   // entries of non-DMVR CUs stay zero, like m_dmvrMvCache users expect
   if (lf) lf_tables(A.lf, p->lfSlices, p->numLfSlices, p->lfSeq);
+  A.lfd.numCus = lfd ? p->numLfCus : 0;
+  if (lfd) {
+    A.lfd.anyDisabled = false;
+    for (int k = 0; k < p->numLfSlices; k++) A.lfd.anyDisabled = A.lfd.anyDisabled || p->lfSlices[k].disable;
+    A.lfd.geom = g; A.lfd.map[1] = A.lfd.map[0] + n4; A.lfd.pus = A.mc.pus; A.lfd.numPus = p->numPus; A.lfd.lfV = const_cast<b200_lf_param*>(A.lf.lfV); A.lfd.lfH = const_cast<b200_lf_param*>(A.lf.lfH);
+  }
   A.lf.dirs = 3;
   if (sao) { if (p->vb) A.sao.vb = *p->vb; else memset(&A.sao.vb, 0, sizeof(A.sao.vb)); }
   for (int k = 0; k < 3; k++) A.mc.refStride[k] = g.stride[k];
@@ -261,6 +277,7 @@ B200_API int b200_pic_upload(b200_ctx* c, const b200_picture* p)
   if (int rc = launch_ctu_validate(A.sao.ctus, A.alf.ctus, A.lf.ctuSlice, (int)nCtu, ctu_limits(g, alf ? p->alfTabs : nullptr, p->numLfSlices), meta, s, h)) return rc;
   if (int rc = launch_intra_validate(A.intra.tus, ni, g, meta, s, h)) return rc;
   if (A.lmcsChromaAdj) if (int rc = launch_lmcs_validate(A.lm.vpdus, g, meta, s, h)) return rc;
+  if (lfd) if (int rc = launch_lf_validate(A.lfd.cus, p->numLfCus, A.lfd.tus, p->numLfTus, A.lfd.ctuCus, g, p->numLfSlices, meta, s, h)) return rc;
   B200_CUDA(cudaMemcpyAsync(A.hMeta, meta, 2 * LM_INTS * sizeof(int), cudaMemcpyDeviceToHost, s));   // list lengths for b200_pic_run's grids
   B200_CUDA(cudaEventRecord(A.uploaded, s));
   return ai;
@@ -280,6 +297,7 @@ B200_API int b200_pic_run(b200_ctx* c, int ai)
   B200_CHECK(!(A.hMeta[LM_ERR] & 8), "b200_pic_run: an intra block record is invalid (geometry, mode, or availability reaching outside the picture)");
   B200_CHECK(!(A.hMeta[LM_ERR] & 4), "b200_pic_run: a CTU record (SAO type / band, ALF filter index or clip / pad flags, slice index) is out of range");
   B200_CHECK(!(A.hMeta[LM_ERR] & 16), "b200_pic_run: an LMCS VPDU record is invalid (CU origin outside the picture or not at or above-left of its VPDU in the same CTU, or an available neighbour outside the picture)");
+  B200_CHECK(!(A.hMeta[LM_ERR] & LM_ERR_LF_RECORD), "b200_pic_run: a CU / TU record of the edge derivation is invalid (block outside its plane or CTU, slice or TU index out of range, CTU ranges)");
   B200_CHECK(!A.hMeta[LM_INTS + LM_ERR], "b200_pic_run: the picture's TU list holds an invalid record");
   B200_CUDA(cudaStreamWaitEvent(s, A.uploaded, 0));
   const b200_geom& g = c->g;
@@ -327,6 +345,7 @@ B200_API int b200_pic_run(b200_ctx* c, int ai)
   // 3. K3 deblocking
   if (A.flags & B200_PIC_DEBLOCK) {
     A.lf.planes = P;
+    if (A.lfd.numCus) if (int rc = launch_lf_derive(A.lfd, s, h)) return rc;
     if (int rc = launch_lf_deblock(A.lf, s, h)) return rc;
   }
   // 4. K4 SAO (out of place)

@@ -207,6 +207,37 @@ __host__ __device__ inline const char* lmcs_vpdu_problem(const b200_lmcs_vpdu& v
   return nullptr;
 }
 
+// ---- B200_PIC_DERIVE_LF: CU and TU records (b200_lf_cu, b200_lf_tu) ----
+// lf_derive.cuh writes grid entries inside a CU's blocks and its TUs' blocks only, and reads the records a CU and TU index name: each CU record and its TUs
+// must lie inside the planes they address and inside the CTU whose range lists the CU (ctu: raster index; the CTU is what calcFilterStrengthsCTU's early
+// return at a slice with deblocking disabled applies to), slice and TU indices inside their arrays.
+struct LfLimits { int W, H, chroma, ctuLog2, ctusW, numSlices; unsigned numTus; };
+inline LfLimits lf_limits(const b200_geom& g, int numSlices, size_t numTus)
+{
+  LfLimits l; l.W = g.width; l.H = g.height; l.chroma = g.chromaFormat != 0; l.ctuLog2 = ctu_log2(g); l.ctusW = (g.width + g.ctuSize - 1) / g.ctuSize;
+  l.numSlices = numSlices; l.numTus = (unsigned)(numTus > 0xffffffffu ? 0xffffffffu : numTus);
+  return l;
+}
+// block (x, y, w, h) of channel type ch inside its plane and inside CTU ctu
+__host__ __device__ inline bool lf_block_in_ctu(int x, int y, int w, int h, int ch, int ctu, const LfLimits& lim)
+{
+  const int cl = lim.ctuLog2 - ch, pw = ch ? lim.W >> 1 : lim.W, ph = ch ? lim.H >> 1 : lim.H;
+  return w >= 1 && h >= 1 && x + w <= pw && y + h <= ph && (x >> cl) == ctu % lim.ctusW && (y >> cl) == ctu / lim.ctusW && ((x + w - 1) >> cl) == (x >> cl) && ((y + h - 1) >> cl) == (y >> cl);
+}
+__host__ __device__ inline const char* lf_cu_problem(const b200_lf_cu& c, const b200_lf_tu* tus, int ctu, const LfLimits& lim)
+{
+  if (c.chType > 1 || (c.chType && !lim.chroma) || c.treeType > 2 || (c.flags & ~0x7ff)) return "CU record: channel, tree type or flags";
+  if (!lf_block_in_ctu(c.x, c.y, c.w, c.h, c.chType, ctu, lim)) return "CU record: block outside its plane or its CTU";
+  if (c.slice >= lim.numSlices) return "CU record: slice index past numLfSlices";
+  if (!c.numTus || (unsigned long long)c.firstTu + c.numTus > lim.numTus) return "CU record: TU records past numLfTus";
+  for (unsigned k = 0; k < c.numTus; k++) {
+    const b200_lf_tu& t = tus[c.firstTu + k];
+    if ((t.w || t.h) && !lf_block_in_ctu(t.x, t.y, t.w, t.h, 0, ctu, lim)) return "TU record: luma block outside the picture or its CU's CTU";
+    if ((t.cw || t.ch) && (!lim.chroma || !lf_block_in_ctu(t.cx, t.cy, t.cw, t.ch, 1, ctu, lim))) return "TU record: chroma block outside the picture or its CU's CTU";
+  }
+  return nullptr;
+}
+
 // ---- K3: the reach of each side of one luma edge ----
 // len is the signalled length (1, 2, 3, 5 or 7).  At a CTU row (ctuRowP: a horizontal edge on a CTU's top row) the P side is never large, and beside a
 // large side a short one filters as 3.  A side writes at most `writes` samples and reads `reads`: writes + 1, and 3 for lengths 1 and 2, whose decisions

@@ -147,4 +147,46 @@ inline void flattenLfCtu( const CodingStructure& cs, const int ctuRsAddr, const 
   for( int y = 0; y < h; y++ ) memcpy( raster + (size_t) ( y0 + y ) * W4 + x0, src + (size_t) y * c4, sizeof( b200_lf_param ) * w );
 }
 
+// The records of the device edge derivation (B200_PIC_DERIVE_LF) in place of calcFilterStrengthsCTU + flattenLfCtu.  One b200_lf_cu per CU, in cs.traverseCUs
+// order; firstTu / firstPu are where its TU records (flattenLfTu, every TU of the CU) and its first PU record go.  leftEdge / topEdge are
+// LoopFilter::xGetLoopfilterParam's (LoopFilter.cpp:1063), which needs the slice and tile membership only the host has.
+static_assert( sizeof( b200_lf_cu ) == 24 && sizeof( b200_lf_tu ) == 16, "b200_lf_cu / b200_lf_tu sizes are part of the C ABI" );
+inline void flattenLfCu( const CodingUnit& cu, const uint32_t firstTu, const uint32_t numTus, const uint32_t firstPu, const int sliceIdx, b200_lf_cu& r )
+{
+  memset( &r, 0, sizeof( r ) );
+  const ChannelType ch = cu.chType(); const CompArea& a = cu.blocks[ch];
+  const PPS& pps = *cu.pps; const SPS& sps = *cu.sps;
+  r.x = (uint16_t) a.x; r.y = (uint16_t) a.y; r.w = (uint8_t) a.width; r.h = (uint8_t) a.height;
+  r.chType = (uint8_t) ch; r.treeType = (uint8_t) cu.treeType();
+  uint16_t f = 0;
+  if( CU::isIntra( cu ) ) f |= B200_LF_CU_INTRA;
+  if( cu.ciipFlag() ) f |= B200_LF_CU_CIIP;
+  if( cu.affineFlag() ) f |= B200_LF_CU_AFFINE;
+  if( cu.mergeFlag() && cu.mergeType() == MRG_TYPE_SUBPU_ATMVP ) f |= B200_LF_CU_SBTMVP;
+  if( cu.geoFlag() ) f |= B200_LF_CU_GEO;
+  if( cu.ispMode() ) f |= B200_LF_CU_ISP;
+  if( cu.bdpcmMode() ) f |= B200_LF_CU_BDPCM_Y;
+  if( cu.bdpcmModeChroma() ) f |= B200_LF_CU_BDPCM_C;
+  if( CU::isSepTree( cu ) ) f |= B200_LF_CU_SEP_TREE;
+  auto avail = [&]( const Position p ) {
+    const CodingUnit* n = cu.cs->getCU( p, ch );
+    const bool sub = !sps.getSubPicInfoPresentFlag() || ( pps.getSubPicFromCU( cu ).getloopFilterAcrossSubPicEnabledFlag() && pps.getSubPicFromCU( *n ).getloopFilterAcrossSubPicEnabledFlag() );
+    return CU::isAvailable( cu, *n, !pps.getLoopFilterAcrossSlicesEnabledFlag(), !pps.getLoopFilterAcrossTilesEnabledFlag(), !sub );
+  };
+  if( a.x > 0 && avail( a.pos().offset( -1, 0 ) ) ) f |= B200_LF_CU_AVAIL_LEFT;
+  if( a.y > 0 && avail( a.pos().offset( 0, -1 ) ) ) f |= B200_LF_CU_AVAIL_TOP;
+  r.flags = f;
+  r.qp = (int8_t) cu.qp; r.slice = (uint8_t) sliceIdx;
+  if( cu.geoFlag() ) r.geoLists = (uint8_t) ( ( ( cu.interDirrefIdxGeo0() >> 4 ) == 2 ? 1 : 0 ) | ( ( cu.interDirrefIdxGeo1() >> 4 ) == 2 ? 2 : 0 ) );
+  r.numTus = (uint8_t) numTus; r.firstTu = firstTu; r.firstPu = firstPu;
+}
+inline void flattenLfTu( const TransformUnit& tu, b200_lf_tu& r )
+{
+  memset( &r, 0, sizeof( r ) );
+  const CompArea& y = tu.blocks[COMPONENT_Y];
+  r.x = (uint16_t) y.x; r.y = (uint16_t) y.y; r.w = (uint8_t) y.width; r.h = (uint8_t) y.height;
+  if( tu.blocks.size() > 1 ) { const CompArea& c = tu.blocks[COMPONENT_Cb]; r.cx = (uint16_t) c.x; r.cy = (uint16_t) c.y; r.cw = (uint8_t) c.width; r.ch = (uint8_t) c.height; }
+  r.cbf = tu.cbf; r.jointCbCr = tu.jointCbCr; r.chromaQp[0] = tu.chromaQp[0]; r.chromaQp[1] = tu.chromaQp[1];
+}
+
 }   // namespace b200glue
